@@ -57,7 +57,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -237,6 +237,8 @@ def run_knn(args, L, dev, rank, world, barrier):
 
     launches0 = L.dbx_kernel_launch_count()
     (ms_dev, gemm_ms), res = timed(q_dev, args.steps, args.warmup)
+    if rank == 0 and args.dump_outputs:
+        dump_arrays(args.dump_outputs, {"knn_idx": np.asarray(res[0], np.float64), "knn_dist": np.asarray(res[1], np.float32)})
     launches = L.dbx_kernel_launch_count() - launches0
     (ms_host, _), _ = timed(q_host, max(1, min(args.steps, 3)), 1)
     stats = op.stats()
@@ -244,10 +246,10 @@ def run_knn(args, L, dev, rank, world, barrier):
     if rank != 0:
         return None
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak, src = 1400.0, "fallback (B200_PROFILING.md sustained)"
+    peak, src = 989.0, "H100 SXM data sheet (dense BF16), not measured"
     if os.path.exists(p):
         with open(p) as f:
-            peak, src = json.load(f).get("bf16_tflops_sustained", 1400.0), "measured sustained cuBLAS bf16 (MEASURED_PEAKS.json)"
+            peak, src = json.load(f).get("bf16_tflops_sustained", 989.0), "measured sustained cuBLAS bf16 (MEASURED_PEAKS.json)"
     flop = 2.0 * nq * n * dim  # per rank and batch: the similarity GEMM (SURVEY 8d row 5)
     achieved = flop / (gemm_ms * 1e-3) / 1e12
     out = {
@@ -281,6 +283,39 @@ def run_knn(args, L, dev, rank, world, barrier):
         out["cpu_baseline"] = {"value": sq / dt * sn / n_total, "unit": "queries/s", "cores": threads, "kind": "port",
                                "sample": f"{sq} queries x {sn} rows, row-wise cosine_distance (oracle, OpenMP) + top-k, scaled by {sn}/{n_total} rows"}
     return out
+
+# ---------------------------------------------------------------------------------- output dump
+DUMP_AGG_MAX_ROWS = 1_900_000  # 4 float64 columns: ~61 MB, under the 64 MB budget of one dump
+
+
+def agg_result_arrays(L, dev, block):
+    """The result block of the last timed step ([sum(v), count(v), avg(x), k], device-resident),
+    copied to the host and ordered by k, as float64 arrays (every value is exact in float64 for
+    this workload: |sum(v)| < 2^53).  Beyond DUMP_AGG_MAX_ROWS groups a fixed, seeded sample of
+    the key-ordered rows is kept."""
+    import numpy as np
+    from databend_b200 import abi, lib
+    np_types = {abi.I64: np.int64, abi.U64: np.uint64, abi.F64: np.float64}
+    cols = []
+    for i in range(block.num_cols):
+        c = block.cols[i]
+        a = np.empty(c.len, dtype=np_types[c.dtype])
+        if c.len:
+            lib.check(L.dbx_memcpy_d2h(dev, a.ctypes.data, c.data, a.nbytes))
+        cols.append(a)
+    order = np.argsort(cols[3], kind="stable")
+    if len(order) > DUMP_AGG_MAX_ROWS:
+        order = order[np.sort(np.random.default_rng(0).choice(len(order), DUMP_AGG_MAX_ROWS, replace=False))]
+    names = ["agg_sum_v", "agg_count_v", "agg_avg_x", "agg_key"]
+    return {nm: cols[i][order].astype(np.float64) for i, nm in enumerate(names)}
+
+
+def dump_arrays(out_dir, arrays):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
 
 # ---------------------------------------------------------------------------------- GPU arm
 def verify_result(out_block, dev, rank, world, cols, n, keys_total, torch, dist):
@@ -502,7 +537,7 @@ def run_dbx(args):
             dist.barrier()
         torch.cuda.synchronize()
 
-    def run_steps(blocks, steps, out_mem, timed):
+    def run_steps(blocks, steps, out_mem, timed, keep_last=None):
         res = None
         for i in range(steps):
             res = step_device(blocks, out_mem, prefetch_next=(i + 1 < steps))
@@ -510,7 +545,10 @@ def run_dbx(args):
                 step_walls.append(time.perf_counter())
             if out_mem == abi.MEM_DEVICE:
                 rows_out = res.num_rows
-                L.dbx_block_release(C.byref(res))
+                if keep_last is not None and i + 1 == steps:
+                    keep_last.append(res)  # released by the caller, after the timed region
+                else:
+                    L.dbx_block_release(C.byref(res))
                 res = rows_out
         return res
 
@@ -528,7 +566,8 @@ def run_dbx(args):
     ev1 = torch.cuda.Event(enable_timing=True)
     ev0.record(part_stream)
     t0 = time.perf_counter()
-    groups = run_steps([dblock], args.steps, abi.MEM_DEVICE, True)
+    last_result = [] if (args.dump_outputs and rank == 0) else None
+    groups = run_steps([dblock], args.steps, abi.MEM_DEVICE, True, keep_last=last_result)
     ev1.record(fin_stream)
     barrier()
     wall = time.perf_counter() - t0
@@ -536,6 +575,9 @@ def run_dbx(args):
     gc.enable()
     dev_ms = ev0.elapsed_time(ev1)
     clocks = sampler.stop() if rank == 0 else None
+    if last_result:
+        dump_arrays(args.dump_outputs, agg_result_arrays(L, dev, last_result[0]))
+        L.dbx_block_release(C.byref(last_result[0]))
     launches = L.dbx_kernel_launch_count() - launches0
     step_ms = max(dev_ms, 0.0) / args.steps
     t = torch.tensor([step_ms, wall * 1e3 / args.steps], dtype=torch.float64, device=f"cuda:{dev}")
@@ -659,7 +701,7 @@ def run_dbx(args):
         "config": {"workload": "configs[1]: filter(v%3=0) + hash-agg sum(v),count(v),avg(x) GROUP BY k; 1e6 int64 keys",
                    "rows": total_rows, "rows_per_gpu": n, "groups_out": verify["groups"] if verify else None,
                    "groups_out_rank0": int(groups),
-                   "columns": "k:int64 v:int64 x:float64", "l2": "inputs (24 B/row x rows) far larger than the 126 MB L2",
+                   "columns": "k:int64 v:int64 x:float64", "l2": "inputs (24 B/row x rows) far larger than the 50 MB L2",
                    "timing": "CUDA events on the operators' streams around the K steps, max over ranks; wall_ms_per_step alongside",
                    "pipelining": ("partial operator scans query i+1 while the final operator merges/materialises query i (every query's work inside the timed region)" if pipeline else "none"),
                    "per_step_wall_ms": {"min": float(per_step.min()), "median": float(np.median(per_step)), "max": float(per_step.max())},
@@ -698,6 +740,9 @@ def main():
     ap.add_argument("--knn-queries", type=int, default=1024)
     ap.add_argument("--knn-k", type=int, default=10)
     ap.add_argument("--knn-cpu-rows", type=int, default=1_000_000, help="corpus rows of the CPU sample in the reference arm")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy "
+                         "(aggregate result ordered by key; kNN row ids and distances of the query batch)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's DataBlock / BlockEntry / Column / Bitmap.
 
-Reference types (paths relative to /root/reference):
+Reference types (paths relative to the databend source tree):
   DataBlock{entries, num_rows, meta}      src/query/expression/src/block.rs:49-60
   BlockEntry::{Const, Column}             src/query/expression/src/block.rs:62-80
   Column::Number / Nullable / Vector      src/query/expression/src/values.rs:192-215

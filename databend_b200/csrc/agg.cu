@@ -1,7 +1,7 @@
 // agg.cu — DBX_OP_AGG_PARTIAL / DBX_OP_AGG_FINAL: host side of the fused
 // [TransformFilter ->] TransformPartialAggregate -> TransformFinalAggregate path.
 //
-// Reference operators replaced (paths relative to /root/reference):
+// Reference operators replaced (paths relative to the databend source tree):
 //   TransformFilter                    src/query/pipeline/transforms/src/processors/transforms/filters/filter_predicate.rs:35-104
 //   TransformPartialAggregate          src/query/service/src/pipelines/processors/transforms/aggregator/transform_aggregate_partial.rs:117-304
 //   PartialSingleStateAggregator       .../aggregator/transform_single_key.rs:42-188
@@ -20,7 +20,7 @@ namespace dbx {
 namespace {
 
 constexpr int64_t kChunkRows = 1LL << 28;        // rows per kernel launch (u32 overflow row ids)
-constexpr int64_t kDefaultTableBytes = 64 << 20; // default table = half of the 126 MB L2
+constexpr int64_t kDefaultTableBytes = 64 << 20; // default table: 1e6 groups of config 2's shape without growth
 constexpr int kProbeLimit = 64;  // buckets (x4 slots)
 constexpr uint32_t kDefaultBulkLanes = 0x6DB6DB6Du;  // 21 of 32 lanes on the TMA unit
 
@@ -383,12 +383,10 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
   // bound by L2 atomic operations per row, not by bytes).
   for (int w = 0; w < kMaxWords; ++w) { pl->w_pair[w] = -1; pl->w_pos[w] = 0; }
   pl->n_pairs = 0;
-  // Measured on B200 (profiles/r02_agg_lane_sweep.txt): the TMA bulk-reduction path does NOT lift
-  // the bound — a 16-byte bulk reduction is split into two 8-byte L2 atomic operations, and the L2
-  // atomic units (~157 G op/s chip-wide) are what the kernel is bound by; every lane split between
-  // TMA and REDs lands on the same 8.05 ms as the plain RED kernel (7.92 ms with the L2 window).
-  // The pair layout and the ring kernel therefore stay opt-in (DBX_AGG_BULK=1) as a documented
-  // negative result; the default is one RED per state word.
+  // The TMA bulk-reduction path does not lift the bound: a 16-byte bulk reduction is split into
+  // two 8-byte L2 atomic operations, and the L2 atomic units are what the kernel is bound by.
+  // The pair layout and the ring kernel therefore stay opt-in (DBX_AGG_BULK=1); the default is
+  // one RED per state word.
   const char* bulk_env = getenv("DBX_AGG_BULK");
   if (pl->grouped && bulk_env && atoi(bulk_env) != 0) {
     for (int cls = 0; cls < 2 && pl->n_pairs < kMaxPairs; ++cls) {
@@ -410,8 +408,7 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
       }
     }
   }
-  // Lane split between the TMA unit and the RED path, measured with experiments/agg_sweep.py
-  // (profiles/r02_agg_lane_sweep.txt).
+  // Lane split between the TMA unit and the RED path (experiments/agg_sweep.py sweeps it).
   pl->bulk_lanes = getenv("DBX_AGG_BULK_LANES") ? (uint32_t)strtoul(getenv("DBX_AGG_BULK_LANES"), nullptr, 16) : kDefaultBulkLanes;
   pl->use_ring = !(getenv("DBX_AGG_RING") && atoi(getenv("DBX_AGG_RING")) == 0);
   pl->debug_flags = getenv("DBX_AGG_DEBUG") ? atoi(getenv("DBX_AGG_DEBUG")) : 0;
@@ -745,8 +742,8 @@ class AggPartialOp : public Op {
     // paired words are updated with plain REDs
     if (FAST && !INDIRECT && kp.n_pairs > 0 && plan.use_ring && ring_ok) return launch_ring<NS>(kp);
     if (FAST && !INDIRECT && kp.n_pairs > 0 && getenv("DBX_AGG_BULK_OLD")) return launch_kernel<NS, FAST, INDIRECT, true, 4>(kp);
-    // (occupancy sweep, profiles/r01b_agg_occupancy_sweep.txt: 4 CTAs/SM at 62 registers is the optimum;
-    // 5-6 CTAs spill and queue up behind the L2 atomics, 2-3 CTAs hide less latency)
+    // (4 CTAs/SM at 62 registers: 5-6 CTAs spill and queue up behind the L2 atomics, 2-3 CTAs hide
+    // less latency)
     return launch_kernel<NS, FAST, INDIRECT, false, 4>(kp);
   }
   template <int NS, bool FAST, bool INDIRECT, bool BULK, int MINB>
@@ -981,8 +978,9 @@ class AggPartialOp : public Op {
   bool no_filter_ = false;
   DevBuf part_buf[kMaxSlots], part_cnt;
   PinnedBuf part_host;
-  int64_t part_threshold = getenv("DBX_AGG_PARTITION_BYTES") ? atoll(getenv("DBX_AGG_PARTITION_BYTES")) : (96LL << 20);
-  int64_t part_region_bytes = getenv("DBX_AGG_REGION_BYTES") ? atoll(getenv("DBX_AGG_REGION_BYTES")) : (48LL << 20);
+  // defaults sized to the 50 MB L2: tables beyond ~80% of it go two-pass, in regions of ~40% of it
+  int64_t part_threshold = getenv("DBX_AGG_PARTITION_BYTES") ? atoll(getenv("DBX_AGG_PARTITION_BYTES")) : (40LL << 20);
+  int64_t part_region_bytes = getenv("DBX_AGG_REGION_BYTES") ? atoll(getenv("DBX_AGG_REGION_BYTES")) : (20LL << 20);
   int64_t partitioned_chunks = 0, partition_fallbacks = 0;
   static constexpr int64_t kPartChunkRows = 1LL << 28;
   bool partition_eligible(const DevCol* cols, int64_t m) const {

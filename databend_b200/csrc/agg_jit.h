@@ -4,7 +4,7 @@
 // dynamic `dyn AggregateFunction`s, aggregate_function.rs); the precompiled kernels here interpret
 // a by-value plan per ROW (op if-chains, slot selects, runtime-constant modulo).  An operator instead
 // asks for a kernel compiled for its plan: the plan is printed as one `constexpr StaticPlan`, NVRTC
-// compiles agg_kernels.cuh against it for sm_100a (once per plan shape and process; ~0.5 s), and the
+// compiles agg_kernels.cuh against it for sm_90a (once per plan shape and process; ~0.5 s), and the
 // cubin is loaded through the runtime's library API.  No NVRTC on the machine, or a failed
 // compilation, leaves the operator on the precompiled kernels — same results, more instructions.
 #pragma once

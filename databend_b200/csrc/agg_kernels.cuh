@@ -1,4 +1,4 @@
-// agg_kernels.cuh — fused [filter ->] hash-aggregate kernels for sm_100a.
+// agg_kernels.cuh — fused [filter ->] hash-aggregate kernels for sm_90a.
 //
 // Replaces, for one pushed DataBlock, the reference's per-block chain
 //   TransformFilter (FilterExecutor::select + take)           filter_executor.rs:82-160
@@ -262,13 +262,14 @@ __device__ __forceinline__ uint64_t canonical_float_key(uint64_t bits) {
 }
 
 // ---------------------------------------------------------------- table
-// 256-bit coherent load of one bucket (4 keys): goes to L2, the point of coherence of the CAS.
+// Coherent load of one 32-byte bucket (4 keys) as two 128-bit loads: goes to L2, the point of
+// coherence of the CAS.
 __device__ __forceinline__ u64x4 ld_bucket(const uint64_t* p) {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   u64x4 r;
-  asm volatile("ld.global.relaxed.gpu.L2::evict_last.v4.b64 {%0, %1, %2, %3}, [%4];"
-               : "=l"(r.x), "=l"(r.y), "=l"(r.z), "=l"(r.w)
-               : "l"(p)
-               : "memory");
+  asm volatile("ld.global.relaxed.gpu.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.x), "=l"(r.y) : "l"(p), "l"(pol) : "memory");
+  asm volatile("ld.global.relaxed.gpu.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.z), "=l"(r.w) : "l"(p + 2), "l"(pol) : "memory");
   return r;
 }
 __device__ __forceinline__ int bucket_match(const u64x4& k, uint64_t key) {
@@ -807,8 +808,8 @@ __global__ void __launch_bounds__(kBlock, 4) filter_partition_kernel(const __gri
 
 // ---------------------------------------------------------------- fused kernel, ring variant
 // Same front end as the FAST kernel above; the table phase differs in how the state words are
-// updated.  The plain kernel is bound by the NUMBER of L2 reduction requests (~150 G RED/s
-// chip-wide, profiles/r01b_atomics_microbench.txt), three per surviving row for config 2.  Here
+// updated.  The plain kernel is bound by the NUMBER of L2 reduction requests (experiments/
+// atomics_bench.cu), three per surviving row for config 2.  Here
 // adjacent additive words (e.g. {row count, wrapping integer sum}) are one 16-byte pair and a
 // share of the lanes updates the pair with ONE TMA bulk reduction (cp.reduce.async.bulk, a
 // separate unit that sustains ~1 small op / 5 clk / SM) while the other lanes keep using REDs,

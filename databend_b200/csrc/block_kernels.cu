@@ -1,6 +1,6 @@
 // block_kernels.cu — DataBlock::take / take_ranges / scatter / concat on the device.
 //
-// Reference kernels replaced (paths relative to /root/reference/src/query/expression/src/kernels):
+// Reference kernels replaced (paths relative to the databend source tree, src/query/expression/src/kernels):
 //   DataBlock::take(indices)              take.rs:43-60        (gather by u32 row indices)
 //   DataBlock::take_ranges(ranges, n)     take_ranges.rs:40    (concatenation of row ranges)
 //   DataBlock::scatter(indices, n)        scatter.rs:21        (row i goes to block indices[i], order kept)

@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers for libdbx (sm_100a only).
+// common.cuh — shared host/device helpers for libdbx (sm_90a only).
 #pragma once
 #ifdef __CUDACC_RTC__  // run-time specialised kernels (agg_jit.cu): no host headers under NVRTC
 typedef signed char int8_t;
@@ -25,7 +25,7 @@ typedef unsigned long long uintptr_t;
 
 namespace dbx {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+constexpr int kNumSMs = 132;  // H100 SXM; grids are sized in multiples of this
 
 #ifndef DBX_DEVICE_ONLY
 // ---------------------------------------------------------------- error plumbing
@@ -91,8 +91,8 @@ struct DevCol {
 // ---------------------------------------------------------------- device helpers
 #ifdef __CUDACC__
 
-// L2 cache policies (sm_100a: the plain .L2::evict_* qualifiers are only legal on 256-bit
-// loads; every other width takes a createpolicy descriptor through .L2::cache_hint).
+// L2 cache policies (sm_90a has no .L2::evict_* qualifier on plain loads: every load takes a
+// createpolicy descriptor through .L2::cache_hint).
 __device__ __forceinline__ uint64_t make_policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -105,13 +105,21 @@ __device__ __forceinline__ uint64_t make_policy_evict_last() {
 }
 
 // Streaming loads: read-only path, no L1 allocation, evict-first in L2 so the column stream
-// does not push the hash table out of the 126 MB L2.
+// does not push the hash table out of the 50 MB L2.
 struct u64x4 { uint64_t x, y, z, w; };
-__device__ __forceinline__ u64x4 ld_stream_256(const void* p) {  // LDG.E.NA.EFL2.256.CONSTANT
+__device__ __forceinline__ uint64_t policy_evict_first_hoistable() {  // not volatile: loops share one policy
+  uint64_t p;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// 32 bytes as two 128-bit loads (sm_90a has no 256-bit load)
+__device__ __forceinline__ u64x4 ld_stream_256(const void* p) {
+  const uint64_t pol = policy_evict_first_hoistable();
   u64x4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0, %1, %2, %3}, [%4];"
-               : "=l"(r.x), "=l"(r.y), "=l"(r.z), "=l"(r.w)
-               : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.x), "=l"(r.y) : "l"(p), "l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;"
+               : "=l"(r.z), "=l"(r.w)
+               : "l"((const char*)p + 16), "l"(pol));
   return r;
 }
 __device__ __forceinline__ uint4 ld_stream_128(const void* p, uint64_t pol) {

@@ -1,6 +1,6 @@
 // eval.cu — dbx_eval_scalar: Evaluator::run over a DataBlock for numeric expressions.
 //
-// Reference replaced (paths relative to /root/reference):
+// Reference replaced (paths relative to the databend source tree):
 //   Evaluator::{run, partial_run, eval_common_call, run_cast}   src/query/expression/src/evaluator.rs:247-465
 //   ScalarFunction::eval + passthrough_nullable                  src/query/expression/src/function.rs:103, register.rs
 //   plus / minus / multiply / divide / div / modulo              src/query/functions/src/scalars/numeric_basic_arithmetic/src/numeric_basic_arithmetic.rs:255-520

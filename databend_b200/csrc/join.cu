@@ -1,15 +1,15 @@
 // join.cu — DBX_OP_JOIN: inner hash join on one integer key column.
 //
-// Reference replaced (paths relative to /root/reference/src/query/service/src/pipelines/processors/transforms):
+// Reference replaced (paths relative to the databend source tree, src/query/service/src/pipelines/processors/transforms):
 //   Join trait (add_block / final_build / probe_block -> JoinStream / final_probe)   new_hash_join/join.rs:26-53
 //   TransformHashJoin stage machine Build -> BuildFinal -> Probe                    new_hash_join/transform_hash_join.rs:39-230
 //   BasicHashJoin::{add_block, final_build}                                         new_hash_join/memory/basic.rs:77-160
 //   HashJoinHashTable::{with_build_row_num, insert, probe}                          hash_join_table/hashjoin_hashtable.rs:95-190
 //   InnerHashJoin::probe_block / InnerHashJoinStream::next                          new_hash_join/memory/inner_join.rs:122-262
 //
-// B200 design.  Build rows stay in HBM as columns.  The table is an open-addressed multimap of
-// 32-byte entries {key, build_row + 1 | validity flags, payload0, payload1} = one sector = one
-// 256-bit load: the probe of a row with up to two 8-byte build columns next to the key touches
+// Design.  Build rows stay in HBM as columns.  The table is an open-addressed multimap of
+// 32-byte entries {key, build_row + 1 | validity flags, payload0, payload1} = one sector = two
+// 128-bit loads: the probe of a row with up to two 8-byte build columns next to the key touches
 // ONE random sector (the reference reads an 8-byte header, then chases the entry chain, then
 // gathers the build row).  A 1e9-row probe into a 1e7-row build side is bound by HBM's
 // random-sector rate, not by bytes: every avoided gather is worth as much as the probe itself.
@@ -164,8 +164,11 @@ __device__ __forceinline__ void copy_value(const JoinColDev& c, int64_t src_row,
 // same-address atomics per block and was the bottleneck), (3) writes the first match from
 // registers and re-walks the sequence only for rows with several matches.
 __device__ __forceinline__ JoinEntry load_entry(const JoinEntry* e) {
-  JoinEntry r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_last.v4.b64 {%0, %1, %2, %3}, [%4];" : "=l"(r.key), "=l"(r.row1), "=l"(r.p0), "=l"(r.p1) : "l"(e));
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  JoinEntry r;  // 32 bytes as two 128-bit loads (sm_90a has no 256-bit load)
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.key), "=l"(r.row1) : "l"(e), "l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.p0), "=l"(r.p1) : "l"((const char*)e + 16), "l"(pol));
   return r;
 }
 __device__ __forceinline__ void emit_match(const JoinProbeParams& p, int64_t r, const JoinEntry& e, int64_t pos) {
@@ -525,11 +528,9 @@ class JoinOp : public Op {
     n_part = 1;
     {
       const int64_t bytes = table_cap * (int64_t)sizeof(JoinEntry);
-      // Radix regions are OFF by default: measured on B200 (profiles/r02_ops_n1_after_rework.jsonl and
-      // call F), 1e9 x 1e7 rows: 39.5 ms without regions vs 50.3 ms with 32 MB regions — once the
-      // probe stops at its first match (unique build keys) one random HBM sector per row costs less
-      // than the extra partition pass over the probe block.  DBX_JOIN_REGION_BYTES=<bytes> turns
-      // them on (tests exercise both).
+      // Radix regions are OFF by default: once the probe stops at its first match (unique build
+      // keys) one random HBM sector per row costs less than the extra partition pass over the
+      // probe block.  DBX_JOIN_REGION_BYTES=<bytes> turns them on (tests exercise both).
       int64_t target = 0;
       if (const char* e = getenv("DBX_JOIN_REGION_BYTES")) target = atoll(e);
       if (target > 0 && bytes > 3 * target) {

@@ -1,7 +1,7 @@
 // knn.cu — dbx_eval_distance (row-wise cosine_distance / l2_distance) and dbx_knn_* (brute-force
 // `ORDER BY distance(c, q) LIMIT k` for a batch of queries).
 //
-// Reference replaced (paths relative to /root/reference):
+// Reference replaced (paths relative to the databend source tree):
 //   cosine_distance / l2_distance            src/common/vector/src/distance.rs:19-35,65-80
 //   calculate_distance (row-wise driver)     src/query/functions/src/scalars/vector.rs:497-556
 //   EvalScalar -> TopN pipeline (SURVEY 3.5) blocks/block_operator.rs:90-98 + top_n/*.rs
@@ -606,7 +606,7 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   int cluster = 1;
   {
     const int n_mblk = round_up(nq, kGemmBM) / kGemmBM;
-    if (n_mblk % 2 == 0) cluster = 2;  // measured on B200: 2 > 1 > 4 > 8 (larger clusters leave SMs idle)
+    if (n_mblk % 2 == 0) cluster = 2;  // halves the corpus-tile traffic per CTA; larger clusters leave SMs idle
     if (const char* e = getenv("DBX_KNN_CLUSTER")) {
       const int c = atoi(e);
       if (c == 1 || c == 2 || c == 4 || c == 8) cluster = c;

@@ -1,13 +1,13 @@
-// knn_kernels.cuh — vector distance kernels for sm_100a.
+// knn_kernels.cuh — vector distance kernels for sm_90a.
 //
 //  (1) exact row-wise cosine / L2 in f32 with the reference's evaluation order
 //      (src/common/vector/src/distance.rs:19-35,65-80; ndarray 0.15.6 unrolled_fold for the
 //      cosine sums) — the ScalarFunction::eval replacement and the re-rank of kNN candidates;
-//  (2) the batched query x corpus similarity GEMM on the 5th-generation tensor cores:
-//      TMA (cp.async.bulk.tensor) -> 128B-swizzled shared memory -> tcgen05.mma (bf16 in, f32
-//      accumulators in TMEM) -> tcgen05.ld epilogue that turns dot products into similarities and
-//      keeps only entries that beat the per-query boundary (the k'-th best so far), i.e. the
-//      score matrix is never written to HBM.
+//  (2) the batched query x corpus similarity GEMM on the Hopper tensor cores:
+//      TMA (cp.async.bulk.tensor, multicast across a cluster) -> 128B-swizzled shared memory ->
+//      wgmma (bf16 in, f32 accumulators in registers) -> epilogue on the accumulator fragment that
+//      turns dot products into similarities and keeps only entries that beat the per-query
+//      boundary (the k'-th best so far), i.e. the score matrix is never written to HBM.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -187,30 +187,26 @@ __global__ void prep_rows_kernel(const float* src, int64_t rows, int dim, int di
   if (max_norm_bits && lane == 0 && wmax > 0.0f) atomicMax(max_norm_bits, __float_as_uint(wmax));
 }
 
-// ---------------------------------------------------------------- tcgen05 GEMM with fused filter
-constexpr int kGemmBM = 128;      // queries per tile      (UMMA M)
-constexpr int kGemmBN = 256;      // corpus rows per tile  (UMMA N)
+// ---------------------------------------------------------------- wgmma GEMM with fused filter
+constexpr int kGemmBM = 128;      // queries per tile: two consumer warpgroups of 64 (wgmma M = 64)
+constexpr int kGemmBN = 128;      // corpus rows per tile  (wgmma N)
 constexpr int kGemmBK = 64;       // bf16 per k-block = 128 bytes = one swizzle row
-constexpr int kGemmStages = 4;
-constexpr int kGemmThreads = 192; // warp 0: TMA, warp 1: MMA (+TMEM alloc), warps 2-5: epilogue
-constexpr int kUmmaK = 16;
-constexpr uint32_t kTmemCols = 512;  // two 256-column accumulators
+constexpr int kGemmStages = 5;
+constexpr int kGemmThreads = 384; // warpgroup 0: TMA (one thread), warpgroups 1-2: wgmma + epilogue
+constexpr int kWgmmaK = 16;
 constexpr uint32_t kStageBytesA = kGemmBM * kGemmBK * 2;
 constexpr uint32_t kStageBytesB = kGemmBN * kGemmBK * 2;
-constexpr int kCandStage = 512;   // staged survivors per epilogue warp
+constexpr int kCandStage = 512;   // staged survivors per consumer warp
 
 struct GemmSmem {
   alignas(1024) uint8_t a[kGemmStages][kStageBytesA];
   alignas(1024) uint8_t b[kGemmStages][kStageBytesB];
   alignas(8) uint64_t full_bar[kGemmStages];
   uint64_t empty_bar[kGemmStages];
-  uint64_t tmem_full_bar[2];
-  uint64_t tmem_empty_bar[2];
-  uint32_t tmem_base;
-  // per epilogue warp: survivors are staged here and written out in coalesced bursts, one
+  // per consumer warp: survivors are staged here and written out in coalesced bursts, one
   // reservation (atomic on the global candidate counter) per burst instead of one per survivor
-  alignas(16) uint64_t stage_key[4][kCandStage];
-  uint32_t stage_row[4][kCandStage];
+  alignas(16) uint64_t stage_key[8][kCandStage];
+  uint32_t stage_row[8][kCandStage];
 };
 
 struct KnnGemmParams {
@@ -239,6 +235,17 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// arrive on the barrier at this offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 ra;\n"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
+      : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
@@ -278,46 +285,43 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n" "barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp layout):
-// start>>4 | LBO(=1, ignored for swizzled K-major)<<16 | SBO(1024 B between 8-row groups)>>4 <<32 |
-// version 1 <<46 | layout SWIZZLE_128B(2) <<61
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma: start>>4 | LBO(=1, ignored for
+// swizzled K-major)<<16 | SBO(1024 B between 8-row groups)>>4 <<32 | layout SWIZZLE_128B(1) <<62.
+// A k-step of 16 bf16 inside the 128-byte swizzle row advances the start address by 32 bytes.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// kind::f16 instruction descriptor: D = f32, A = B = bf16, both K-major, N >> 3, M >> 4
-__device__ __forceinline__ uint32_t make_idesc_bf16(int m, int n) {
-  uint32_t d = 0;
-  d |= 1u << 4;               // c_format = F32
-  d |= 1u << 7;               // a_format = BF16
-  d |= 1u << 10;              // b_format = BF16
-  d |= (uint32_t)(n >> 3) << 17;
-  d |= (uint32_t)(m >> 4) << 24;
-  return d;
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, bf16 in, f32 accumulators in registers, both K-major
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrive (once the MMAs issued so far retire) on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(mask)
-               : "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 __device__ __forceinline__ uint32_t f32_to_ordered32(float f) {
   if (f != f) return 0u;  // NaN: worst similarity
@@ -342,11 +346,12 @@ __device__ __forceinline__ void flush_stage(const uint64_t* skey, const uint32_t
 }
 
 // Persistent, warp-specialised kernel.  A cluster of C CTAs works on C consecutive query blocks
-// against the SAME 256-row corpus tile: every CTA streams its own query tile (A) and 1/C of the
+// against the SAME 128-row corpus tile: every CTA streams its own query tile (A) and 1/C of the
 // corpus tile (B), which TMA multicasts into the shared memory of all C CTAs — so per CTA the
-// L2 -> SM traffic per k-block drops from 16+32 KB to 16+32/C KB (the 1-CTA kernel is bound by
-// exactly that traffic: 96 B/clk/SM at full tensor rate).  Consecutive cluster tiles walk the
-// query blocks first, so a corpus tile is fetched from HBM once and re-read from L2.
+// L2 -> SM traffic per k-block drops from 16+16 KB to 16+16/C KB.  Consecutive cluster tiles walk
+// the query blocks first, so a corpus tile is fetched from HBM once and re-read from L2.
+// Each consumer warpgroup multiplies 64 of the tile's 128 queries with wgmma and filters its
+// accumulator fragment in registers, so the score matrix is never written anywhere.
 template <int C>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
@@ -364,24 +369,17 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
   constexpr int kSliceRows = kGemmBN / C;       // corpus rows this CTA fetches for the whole cluster
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kGemmStages; ++s) { mbar_init(&sm.full_bar[s], 1); mbar_init(&sm.empty_bar[s], C); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&sm.tmem_full_bar[a], 1); mbar_init(&sm.tmem_empty_bar[a], 128); }
+    // a slot is free once both consumer warpgroups of every CTA in the cluster have read it
+    for (int s = 0; s < kGemmStages; ++s) { mbar_init(&sm.full_bar[s], 1); mbar_init(&sm.empty_bar[s], 2 * C); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_q) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_c) : "memory");
   }
-  if (warp == 1) {  // one warp allocates TMEM and later frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   if (C > 1) cluster_sync_all(); else __syncthreads();  // peers' barriers are initialised before anyone signals them
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = sm.tmem_base;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int64_t t = cluster_id; t < n_tiles; t += n_clusters) {
@@ -406,92 +404,83 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one elected lane) =====
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(kGemmBM, kGemmBN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t t = cluster_id; t < n_tiles; t += n_clusters) {
-        mbar_wait(&sm.tmem_empty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)acc * kGemmBN;
-        for (int kb = 0; kb < n_kblk; ++kb) {
-          mbar_wait(&sm.full_bar[stage], phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a_addr = smem_u32(sm.a[stage]), b_addr = smem_u32(sm.b[stage]);
-#pragma unroll
-          for (int k = 0; k < kGemmBK / kUmmaK; ++k) {
-            const uint64_t adesc = make_smem_desc(a_addr + k * kUmmaK * 2);
-            const uint64_t bdesc = make_smem_desc(b_addr + k * kUmmaK * 2);
-            umma_bf16(tmem_d, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          // frees the smem stage once these MMAs retire — in every CTA of the cluster, because
-          // each of them writes a slice of the next fill into this CTA's slot
-          if (C > 1) umma_commit_multicast(&sm.empty_bar[stage], kMask); else umma_commit(&sm.empty_bar[stage]);
-          if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&sm.tmem_full_bar[acc]);  // accumulator complete -> epilogue
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
   } else {
-    // ===== epilogue: TMEM -> registers -> score -> boundary filter -> candidate list =====
-    const int quarter = warp & 3;  // a warp may only touch TMEM lanes [32*(warp%4), +32)
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===== consumers: wgmma into registers -> score -> boundary filter -> candidate list =====
+    const int cw = warp - 4;            // consumer warp 0..7
+    const int wg = cw >> 2;             // queries [64*wg, +64) of the tile
+    const uint32_t tid_wg = threadIdx.x & 127;
     const bool is_l2 = p.kind != DBX_DIST_COSINE;
+    // accumulator fragment of m64nNk16: register 4j + 2h + e holds row 16*(warp%4) + lane/4 + 8h,
+    // column 8j + 2*(lane%4) + e
+    const int col_l = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
     int stage_cnt = 0;  // warp-uniform
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+    auto release = [&](int s) {  // one arrival per consumer warpgroup on slot s of every CTA in the cluster
+      if (tid_wg < (uint32_t)C) {
+        if (C > 1) mbar_arrive_cluster(&sm.empty_bar[s], tid_wg); else mbar_arrive(&sm.empty_bar[s]);
+      }
+    };
     for (int64_t t = cluster_id; t < n_tiles; t += n_clusters) {
       const int m_blk = (int)(t % n_mgrp) * C + (int)cta_rank;
       const int64_t n_blk = t / n_mgrp;
-      const int q = m_blk * kGemmBM + quarter * 32 + lane;
-      const bool q_ok = q < p.nq;
-      const float qq = (q_ok && is_l2) ? p.q_scale[q] : 0.0f;
-      const float bound = q_ok ? p.bound[q] : __int_as_float(0x7f800000);  // +inf: nothing passes
-      mbar_wait(&sm.tmem_full_bar[acc], acc_phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+      int prev = -1;
+      for (int kb = 0; kb < n_kblk; ++kb) {
+        mbar_wait(&sm.full_bar[stage], phase);
+        wgmma_fence();
+        const uint32_t a_addr = smem_u32(sm.a[stage]) + (uint32_t)wg * (64 * kGemmBK * 2), b_addr = smem_u32(sm.b[stage]);
+#pragma unroll
+        for (int k = 0; k < kGemmBK / kWgmmaK; ++k)
+          wgmma_m64n128k16_bf16(acc, make_smem_desc(a_addr + k * kWgmmaK * 2), make_smem_desc(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (prev >= 0) { wgmma_wait<1>(); release(prev); }  // the previous k-block's MMAs are done with their slot
+        prev = stage;
+        if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      release(prev);
+
+      const int q_a = m_blk * kGemmBM + wg * 64 + (cw & 3) * 16 + (lane >> 2);
+      int qs[2];
+      float qq[2], bnd[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        qs[h] = q_a + 8 * h;
+        const bool q_ok = qs[h] < p.nq;
+        qq[h] = (q_ok && is_l2) ? p.q_scale[qs[h]] : 0.0f;
+        bnd[h] = q_ok ? p.bound[qs[h]] : __int_as_float(0x7f800000);  // +inf: nothing passes
+      }
       const int64_t row0 = p.n0 + n_blk * kGemmBN;
-      const int64_t row_end = p.n0 + p.n_rows;
-#pragma unroll 1
-      for (int c = 0; c < kGemmBN / 32; ++c) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * kGemmBN + c * 32);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr)
-            : "memory");
-        const int64_t rbase = row0 + c * 32;
-        const int64_t left = row_end - rbase;  // rows of this chunk that exist
-        const uint32_t col_mask = left >= 32 ? 0xFFFFFFFFu : (left <= 0 ? 0u : ((1u << (int)left) - 1u));
-        float cc_lane = 0.0f;
-        if (is_l2) cc_lane = (lane < left) ? __ldg(p.c_scale + rbase + lane) : 0.0f;
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      const int64_t left = p.n0 + p.n_rows - row0;  // rows of this tile that exist
+#pragma unroll
+      for (int c = 0; c < kGemmBN / 32; ++c) {  // 32 columns per round: 16 scores per thread
+        float sc[16];
         uint32_t pass = 0;
-        if (!is_l2) {
-          // cosine: operands are pre-normalised, the accumulator IS the similarity
 #pragma unroll
-          for (int j = 0; j < 32; ++j) pass |= (__uint_as_float(v[j]) >= bound) ? (1u << j) : 0u;
-        } else {
-          // L2: score = -(|q|^2 + |c|^2 - 2 q.c)   (larger = closer)
+        for (int jj = 0; jj < 4; ++jj) {
+          const int col = (c * 4 + jj) * 8 + col_l;
+          float cc[2] = {0.0f, 0.0f};
+          if (is_l2) {
+            if (col < left) cc[0] = __ldg(p.c_scale + row0 + col);
+            if (col + 1 < left) cc[1] = __ldg(p.c_scale + row0 + col + 1);
+          }
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float cc = __shfl_sync(0xffffffffu, cc_lane, j);
-            const float sc = 2.0f * __uint_as_float(v[j]) - qq - cc;
-            v[j] = __float_as_uint(sc);
-            pass |= (sc >= bound) ? (1u << j) : 0u;
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int idx = jj * 4 + h * 2 + e;
+              float s = acc[(c * 4 + jj) * 4 + h * 2 + e];
+              // cosine: operands are pre-normalised, the accumulator IS the similarity;
+              // L2: score = -(|q|^2 + |c|^2 - 2 q.c)   (larger = closer)
+              if (is_l2) s = 2.0f * s - qq[h] - cc[e];
+              sc[idx] = s;
+              pass |= (s >= bnd[h] && col + e < left) ? (1u << idx) : 0u;
+            }
           }
         }
-        pass &= col_mask;
         if (__any_sync(0xffffffffu, pass != 0)) {
           const int n = __popc(pass);
           int incl = n;
@@ -503,32 +492,32 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
           const int total = __shfl_sync(0xffffffffu, incl, 31);
           const int excl = incl - n;
           if (total > kCandStage / 2) {
-            // dense chunk (loose boundary in the first passes): reserve once per warp, write direct
+            // dense round (loose boundary in the first passes): reserve once per warp, write direct
             unsigned long long base = 0;
             if (lane == 0) base = atomicAdd(p.cand_count, (unsigned long long)total);
             base = __shfl_sync(0xffffffffu, base, 0);
             if ((int64_t)(base + total) <= p.cand_cap) {
               unsigned long long pos = base + excl;
 #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                if ((pass >> j) & 1) {
-                  p.cand_key[pos] = ((uint64_t)(uint32_t)q << 32) | (uint64_t)(~f32_to_ordered32(__uint_as_float(v[j])));
-                  p.cand_row[pos] = (uint32_t)(rbase + j);
+              for (int idx = 0; idx < 16; ++idx) {
+                if ((pass >> idx) & 1) {
+                  p.cand_key[pos] = ((uint64_t)(uint32_t)qs[(idx >> 1) & 1] << 32) | (uint64_t)(~f32_to_ordered32(sc[idx]));
+                  p.cand_row[pos] = (uint32_t)(row0 + (c * 4 + (idx >> 2)) * 8 + col_l + (idx & 1));
                   ++pos;
                 }
               }
             }
           } else {
             if (stage_cnt + total > kCandStage) {
-              flush_stage(sm.stage_key[quarter], sm.stage_row[quarter], stage_cnt, lane, p);
+              flush_stage(sm.stage_key[cw], sm.stage_row[cw], stage_cnt, lane, p);
               stage_cnt = 0;
             }
             int pos = stage_cnt + excl;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if ((pass >> j) & 1) {
-                sm.stage_key[quarter][pos] = ((uint64_t)(uint32_t)q << 32) | (uint64_t)(~f32_to_ordered32(__uint_as_float(v[j])));
-                sm.stage_row[quarter][pos] = (uint32_t)(rbase + j);
+            for (int idx = 0; idx < 16; ++idx) {
+              if ((pass >> idx) & 1) {
+                sm.stage_key[cw][pos] = ((uint64_t)(uint32_t)qs[(idx >> 1) & 1] << 32) | (uint64_t)(~f32_to_ordered32(sc[idx]));
+                sm.stage_row[cw][pos] = (uint32_t)(row0 + (c * 4 + (idx >> 2)) * 8 + col_l + (idx & 1));
                 ++pos;
               }
             }
@@ -537,24 +526,15 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(&sm.tmem_empty_bar[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
-    flush_stage(sm.stage_key[quarter], sm.stage_row[quarter], stage_cnt, lane, p);
+    flush_stage(sm.stage_key[cw], sm.stage_row[cw], stage_cnt, lane, p);
   }
   __syncwarp();
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   if (C > 1) cluster_sync_all(); else __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
 }
 
 // Reference similarity pass on CUDA cores (same bf16 inputs, f32 accumulation, same filter):
-// used by the tests to validate the tcgen05 path (env DBX_KNN_REF_GEMM=1), never by default.
+// used by the tests to validate the wgmma path (env DBX_KNN_REF_GEMM=1), never by default.
 __global__ void knn_ref_filter_kernel(const __nv_bfloat16* q, const __nv_bfloat16* c, const __grid_constant__ KnnGemmParams p) {
   const int64_t total = (int64_t)p.nq * p.n_rows;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {

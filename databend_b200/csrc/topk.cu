@@ -1,6 +1,6 @@
 // sort.cu — DBX_OP_TOPK: `ORDER BY key [ASC|DESC] [NULLS FIRST|LAST] [LIMIT k]` on the device.
 //
-// Reference pipeline replaced (paths relative to /root/reference):
+// Reference pipeline replaced (paths relative to the databend source tree):
 //   TransformSortPartial (per block sort + limit)   src/query/pipeline/transforms/src/processors/transforms/sorts/sort_partial.rs:24-60
 //     DataBlock::sort_with_type / SortCompare       src/query/expression/src/kernels/sort.rs:91-111, sort_compare.rs:197-296
 //   limit-aware k-way merge                         sorts/sort_merge*.rs, sorts/core/{merger,loser_tree}.rs

@@ -67,7 +67,7 @@ def all_to_all_rows(send: torch.Tensor, send_counts: Sequence[int], row_bytes: i
 
 
 class PeerExchange:
-    """Partial -> final shuffle through peer memory (NVLink), the B200-native replacement of the
+    """Partial -> final shuffle through peer memory (NVLink), the GPU-native replacement of the
     all-to-all above: `scatter(partial)` partitions the partial's groups and stores every row
     straight into its owner's receive buffer, `merge(final)` waits on the device for all sources
     and merges.  Only the one-time exchange of the 64-byte IPC handles goes through

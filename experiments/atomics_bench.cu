@@ -1,6 +1,6 @@
-// experiments/atomics_bench.cu — what does B200 give for "stream 24 B/row + random L2 atomics"?
+// experiments/atomics_bench.cu — what does the GPU give for "stream 24 B/row + random L2 atomics"?
 // Variants isolate the stream, the probe load and the REDs of the fused filter->hash-agg kernel.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o atomics_bench atomics_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o atomics_bench atomics_bench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -8,8 +8,11 @@
 
 struct u64x4 { uint64_t x, y, z, w; };
 __device__ __forceinline__ u64x4 ld256(const void* p) {
-  u64x4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0,%1,%2,%3}, [%4];" : "=l"(r.x), "=l"(r.y), "=l"(r.z), "=l"(r.w) : "l"(p));
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  u64x4 r;  // two 128-bit loads: sm_90a has no 256-bit load
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%2], %3;" : "=l"(r.x), "=l"(r.y) : "l"(p), "l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%2], %3;" : "=l"(r.z), "=l"(r.w) : "l"((const char*)p + 16), "l"(pol));
   return r;
 }
 __device__ __forceinline__ uint64_t mix(uint64_t x) {

@@ -1,5 +1,5 @@
 /*
- * dbx.h — C-ABI of libdbx, the B200-native replacement for Databend's in-memory
+ * dbx.h — C-ABI of libdbx, the H100-native replacement for Databend's in-memory
  * vectorised execution hot path (filter -> hash aggregate / hash join / top-k /
  * vector distance).
  *
@@ -463,7 +463,7 @@ int32_t dbx_op_last_kernel_ms(dbx_op* op, float* ms);
  * the kernel of query i can be read after query i+1 was enqueued without waiting for it. */
 int32_t dbx_op_kernel_ms(dbx_op* op, int32_t back, float* ms);
 /* Which build of the hot kernel serves this handle.  Aggregate operators ask for a kernel compiled
- * for their plan at create time (NVRTC, sm_100a; cached per plan shape; DBX_AGG_JIT=0 turns it off):
+ * for their plan at create time (NVRTC, sm_90a; cached per plan shape; DBX_AGG_JIT=0 turns it off):
  * "specialised", or "precompiled kernels (<why>)" when the plan-interpreting kernels serve it.
  * Results are identical either way. */
 int32_t dbx_op_kernel_variant(dbx_op* op, char* out, int32_t cap);

@@ -10,7 +10,7 @@
  * (tests/golden/ JSON files, extracted from the reference's testdata with file:line citations)
  * by tests/test_oracle_golden.py.
  *
- * Each function cites the reference file:line it follows (paths relative to /root/reference).
+ * Each function cites the reference file:line it follows (paths relative to the databend source tree).
  *
  * Third-party arithmetic restated from its published algorithm (not vendored in the reference):
  *   ndarray 0.15.6 (Cargo.lock) `numeric_util::unrolled_fold` — 8 interleaved partial sums —

@@ -1,7 +1,7 @@
 """CPU ORACLE for scalar expressions (test infrastructure only — never imported by the product).
 
 Row-by-row Python restatement of the reference's evaluator for the numeric / boolean functions
-libdbx evaluates on the device.  Each rule cites the file it follows (relative to /root/reference):
+libdbx evaluates on the device.  Each rule cites the file it follows (relative to the databend source tree):
   result types          src/query/codegen/src/writes/arithmetics_type.rs:240-265 (arithmetic_coercion)
   plus/minus/multiply   src/query/functions/src/scalars/numeric_basic_arithmetic/src/numeric_basic_arithmetic.rs:255-400
                         ((a as T) op (b as T), wrapping: release build, Cargo.toml:577)

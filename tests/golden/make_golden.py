@@ -1,6 +1,6 @@
 """Writes tests/golden/*.json: known-answer vectors transcribed from the reference's OWN test
 data (the reference is Rust and cannot be run here, so values are copied by hand from its
-golden files; each case carries the file:line it comes from, relative to /root/reference).
+golden files; each case carries the file:line it comes from, relative to the databend source tree).
 Run:  python tests/golden/make_golden.py
 """
 import json

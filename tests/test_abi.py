@@ -103,7 +103,7 @@ def test_ctypes_mirror_matches_the_header_field_by_field(tmp_path):
 
 def test_runtime_specialisation_compiles_here():
     """NVRTC is dlopen'ed by libdbx; the specialised aggregate kernels of a canned plan must compile
-    for sm_100a in this image (no GPU involved)."""
+    for sm_90a in this image (no GPU involved)."""
     import ctypes as C
     from databend_b200.lib import load
     buf = C.create_string_buffer(4096)

@@ -176,7 +176,7 @@ def test_knn_forced_exact_path(gpu, monkeypatch):
 
 
 def test_knn_tensor_core_pass_matches_cuda_core_reference(gpu, monkeypatch):
-    """The tcgen05 similarity pass and the plain CUDA-core pass over the same bf16 operands must
+    """The wgmma similarity pass and the plain CUDA-core pass over the same bf16 operands must
     nominate candidate sets that give the same answer."""
     rng = np.random.default_rng(11)
     corpus = rng.standard_normal((9000, 200)).astype(np.float32)

@@ -28,6 +28,7 @@ OP_FILTER, OP_AGG_PARTIAL, OP_AGG_FINAL, OP_TOPK, OP_JOIN = range(5)
 
 DIST_COSINE, DIST_L2 = 0, 1
 JOIN_INNER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI, JOIN_LEFT = 0, 1, 2, 3
+JOIN_RIGHT, JOIN_RIGHT_SEMI, JOIN_RIGHT_ANTI, JOIN_FULL = 4, 5, 6, 7
 
 MAX_PRED_NODES = 16
 MAX_AGGS = 8
@@ -157,7 +158,7 @@ EXPORTS = [
     "dbx_host_alloc", "dbx_host_free", "dbx_host_register", "dbx_host_unregister",
     "dbx_device_alloc", "dbx_device_free", "dbx_memcpy_h2d", "dbx_memcpy_d2h", "dbx_memcpy_d2d", "dbx_device_synchronize",
     "dbx_op_create", "dbx_op_destroy", "dbx_op_push", "dbx_op_finish", "dbx_op_pull", "dbx_block_release", "dbx_op_reset", "dbx_op_synchronize",
-    "dbx_join_probe", "dbx_agg_final_merge_partial", "dbx_agg_partial_partition", "dbx_agg_final_merge_rows",
+    "dbx_join_probe", "dbx_join_final_probe", "dbx_agg_final_merge_partial", "dbx_agg_partial_partition", "dbx_agg_final_merge_rows",
     "dbx_agg_exchange_create", "dbx_agg_exchange_local_buffer", "dbx_agg_exchange_connect", "dbx_agg_exchange_scatter",
     "dbx_agg_exchange_merge", "dbx_agg_exchange_destroy", "dbx_agg_exchange_last_error",
     "dbx_hash_partition",

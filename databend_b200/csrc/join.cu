@@ -1,4 +1,5 @@
-// join.cu — DBX_OP_JOIN: inner hash join on one integer key column.
+// join.cu — DBX_OP_JOIN: hash join on one integer key column (INNER, LEFT, LEFT SEMI / ANTI, RIGHT,
+// RIGHT SEMI / ANTI, FULL).
 //
 // Reference replaced (paths relative to the databend source tree, src/query/service/src/pipelines/processors/transforms):
 //   Join trait (add_block / final_build / probe_block -> JoinStream / final_probe)   new_hash_join/join.rs:26-53
@@ -89,6 +90,7 @@ struct JoinProbeParams {
   int64_t n_rows;
   int64_t out_cap;
   unsigned long long* cursor;  // number of matches (may exceed out_cap: then the host retries)
+  uint8_t* matched;            // build-side kinds: one byte per build row, set when a probe row matches it
 };
 
 __device__ __forceinline__ uint64_t load_key(const DevCol& c, int64_t row) {
@@ -278,7 +280,10 @@ __global__ void join_dup_check_kernel(const __grid_constant__ JoinTableDev t, un
 // probe_block + JoinStream::next fused, two probe rows per thread: both rows' entry loads are in
 // flight together (the probe is bound by dependent L2 round trips, not by bytes).  UNIQUE: the
 // build side has no duplicate keys, so a row's walk ends at its first match.
-template <bool UNIQUE>
+// MARK (the build-side kinds RIGHT, RIGHT SEMI, RIGHT ANTI, FULL): every matching entry's build
+// row is marked in p.matched for the final scan.  Racing stores all write 1, so no atomics.  RIGHT
+// then emits like INNER, FULL like LEFT, RIGHT SEMI / ANTI emit nothing here.
+template <bool UNIQUE, bool MARK>
 __global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
   __shared__ unsigned int s_warp[kJoinBlock / 32];
   __shared__ unsigned long long s_base;
@@ -317,6 +322,10 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_co
         if (!go[j]) continue;
         if (e[j].row1 == 0) { go[j] = false; continue; }
         if (e[j].key == k[j]) {
+          if (MARK) {  // read first: a dimension row hit by many facts is written once, not per match
+            uint8_t* m = p.matched + (int64_t)(e[j].row1 & kRowMask) - 1;
+            if (*m == 0) *m = 1;
+          }
           if (n_match[j] == 0) first[j] = e[j];
           ++n_match[j];
           if (UNIQUE) { go[j] = false; continue; }
@@ -330,7 +339,8 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_co
       // semi / anti: the probe row itself is the output, at most once (a NULL key counts as no match)
       if (p.kind == DBX_JOIN_LEFT_SEMI) n_match[j] = n_match[j] ? 1u : 0u;
       else if (p.kind == DBX_JOIN_LEFT_ANTI) n_match[j] = (in_range[j] && n_match[j] == 0) ? 1u : 0u;
-      outer_null[j] = p.kind == DBX_JOIN_LEFT && in_range[j] && n_match[j] == 0;  // preserved row without a match
+      else if (MARK && (p.kind == DBX_JOIN_RIGHT_SEMI || p.kind == DBX_JOIN_RIGHT_ANTI)) n_match[j] = 0;  // marked only
+      outer_null[j] = (p.kind == DBX_JOIN_LEFT || (MARK && p.kind == DBX_JOIN_FULL)) && in_range[j] && n_match[j] == 0;  // preserved row without a match
       if (outer_null[j]) n_match[j] = 1;
     }
     // block-wide exclusive scan of the match counts -> one reservation per CTA and step
@@ -380,6 +390,63 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_co
   }
 }
 
+// Join::final_probe of the build-side kinds: stream the matched map and compact the selected build
+// rows (want = 1: rows matched at least once, RIGHT SEMI; want = 0: rows never matched, RIGHT /
+// RIGHT ANTI / FULL, NULL-key rows included since they were never inserted).  Every build column is
+// gathered by build row from its HBM-resident column; positions are reserved like the probe's: a
+// block-wide scan, then one cursor atomic per CTA and step.  With out_cap = 0 it only counts.
+struct FinalColDev {
+  const void* src;
+  const uint8_t* src_valid;  // one byte per build row, or null (all valid)
+  void* dst;
+  uint8_t* dst_valid;        // one byte per output row, or null
+  int32_t size;
+  int32_t pad;
+};
+struct JoinFinalParams {
+  FinalColDev cols[kMaxJoinCols];
+  int32_t n_cols;
+  int32_t want;
+  const uint8_t* matched;
+  int64_t n_rows;
+  int64_t out_cap;
+  unsigned long long* cursor;
+};
+__global__ void __launch_bounds__(kJoinBlock) join_final_scan_kernel(const __grid_constant__ JoinFinalParams p) {
+  __shared__ unsigned int s_warp[kJoinBlock / 32];
+  __shared__ unsigned long long s_base;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  const int64_t n_iter = (p.n_rows + step - 1) / step;
+  for (int64_t it = 0; it < n_iter; ++it) {
+    const int64_t r = it * step + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool sel = r < p.n_rows && (p.matched[r] != 0) == (p.want != 0);
+    const unsigned int ballot = __ballot_sync(0xffffffffu, sel);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      unsigned int tot = 0;
+      for (int w = 0; w < kJoinBlock / 32; ++w) { const unsigned int c = s_warp[w]; s_warp[w] = tot; tot += c; }
+      s_base = tot ? atomicAdd(p.cursor, (unsigned long long)tot) : 0ULL;
+    }
+    __syncthreads();
+    const int64_t pos = (int64_t)s_base + s_warp[warp] + __popc(ballot & ((1u << lane) - 1u));
+    __syncthreads();
+    if (sel && pos < p.out_cap) {
+      for (int c = 0; c < p.n_cols; ++c) {
+        const FinalColDev& fc = p.cols[c];
+        switch (fc.size) {
+          case 8: ((uint64_t*)fc.dst)[pos] = ((const uint64_t*)fc.src)[r]; break;
+          case 4: ((uint32_t*)fc.dst)[pos] = ((const uint32_t*)fc.src)[r]; break;
+          case 2: ((uint16_t*)fc.dst)[pos] = ((const uint16_t*)fc.src)[r]; break;
+          default: ((uint8_t*)fc.dst)[pos] = ((const uint8_t*)fc.src)[r]; break;
+        }
+        if (fc.dst_valid) fc.dst_valid[pos] = fc.src_valid ? fc.src_valid[r] : 1;
+      }
+    }
+  }
+}
+
 // Pull one table region into L2 with full-line sequential reads before it is probed: the probes
 // themselves would fetch it as scattered 32-byte sectors, which HBM serves an order of magnitude
 // slower than a stream.
@@ -405,6 +472,8 @@ inline int64_t next_pow2_i64(int64_t x) {
   while (p < x) p <<= 1;
   return p;
 }
+// the kinds that keep build rows: they mark matches during the probe and emit from final_probe
+inline bool build_side_kind(int kind) { return kind >= DBX_JOIN_RIGHT && kind <= DBX_JOIN_FULL; }
 inline int grid_rows(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + kJoinBlock - 1) / kJoinBlock, (int64_t)kNumSMs * 8)); }
 
 // Device column that grows by appending pushed blocks (build side).
@@ -444,12 +513,14 @@ class JoinOp : public Op {
   JoinTableDev table_view() const { return JoinTableDev{(JoinEntry*)table_buf.p, table_cap, region, n_part, 0}; }
   std::vector<std::unique_ptr<OwnedBlock>> outputs;  // joined blocks waiting to be pulled (device resident)
   size_t next_out = 0;
+  DevBuf matched;             // build-side kinds: one byte per build row, 1 once any probe row matched it
+  bool final_probed = false;  // Join::final_probe ran: no more probe blocks until reset
 
   // input_types = build schema (params.n_build_cols columns) followed by the probe schema.
   int32_t init(const dbx_join_params* p, const int32_t* types, int32_t n, int dev) {
     DBX_TRY(base_init(dev));
     prm = *p;
-    if (p->kind < DBX_JOIN_INNER || p->kind > DBX_JOIN_LEFT) { err.set("join kind not built (INNER, LEFT, LEFT SEMI and LEFT ANTI are; right/full joins are next, SURVEY 8f.3)"); return DBX_ERR_UNSUPPORTED; }
+    if (p->kind < DBX_JOIN_INNER || p->kind > DBX_JOIN_FULL) { err.set("join: unknown dbx_join_kind"); return DBX_ERR_UNSUPPORTED; }
     n_build_cols = p->n_build_cols;
     n_probe_cols = n - n_build_cols;
     if (n_build_cols <= 0 || n_probe_cols <= 0 || n_build_cols > kMaxJoinCols || n_probe_cols > kMaxJoinCols) {
@@ -553,6 +624,10 @@ class JoinOp : public Op {
     }
     DBX_CUDA_TRY(err, table_buf.ensure((size_t)table_cap * sizeof(JoinEntry)));
     DBX_CUDA_TRY(err, cudaMemsetAsync(table_buf.p, 0, (size_t)table_cap * sizeof(JoinEntry), stream));
+    if (build_side_kind(prm.kind)) {  // the matched map, indexed by build row (NULL-key rows stay 0)
+      DBX_CUDA_TRY(err, matched.ensure((size_t)std::max<int64_t>(build_rows, 1)));
+      DBX_CUDA_TRY(err, cudaMemsetAsync(matched.p, 0, (size_t)std::max<int64_t>(build_rows, 1), stream));
+    }
     if (build_rows) {
       GrowCol& kc = build[prm.build_key_col];
       DevCol key;
@@ -599,15 +674,21 @@ class JoinOp : public Op {
 
   void launch_probe(const JoinProbeParams& pp, int64_t rows) {
     static const bool old_probe = getenv("DBX_JOIN_OLD_PROBE") != nullptr;
-    if (old_probe) { join_probe_kernel<<<grid_rows(rows), kJoinBlock, 0, stream>>>(pp); return; }
     const int grid = grid_rows((rows + 1) / 2);
-    if (build_unique) join_probe2_kernel<true><<<grid, kJoinBlock, 0, stream>>>(pp);
-    else join_probe2_kernel<false><<<grid, kJoinBlock, 0, stream>>>(pp);
+    if (pp.matched) {  // build-side kinds: always the two-row kernel (DBX_JOIN_OLD_PROBE is an ablation of the probe-side kinds)
+      if (build_unique) join_probe2_kernel<true, true><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<false, true><<<grid, kJoinBlock, 0, stream>>>(pp);
+      return;
+    }
+    if (old_probe) { join_probe_kernel<<<grid_rows(rows), kJoinBlock, 0, stream>>>(pp); return; }
+    if (build_unique) join_probe2_kernel<true, false><<<grid, kJoinBlock, 0, stream>>>(pp);
+    else join_probe2_kernel<false, false><<<grid, kJoinBlock, 0, stream>>>(pp);
   }
 
   // Join::probe_block: join one probe block; the joined block is queued for dbx_op_pull
   int32_t probe(const dbx_block* b) {
     if (!finished) { err.set("probe before final_build"); return DBX_ERR_STATE; }
+    if (final_probed) { err.set("probe_block after final_probe (reset the operator first)"); return DBX_ERR_STATE; }
     if (b->num_cols != n_probe_cols) { err.set("probe_block: block does not match the probe schema"); return DBX_ERR_INVALID; }
     const int64_t n = b->num_rows;
     if (n == 0) return DBX_OK;
@@ -618,7 +699,9 @@ class JoinOp : public Op {
       if (col.dtype != probe_dtype[c] || col.len != n || col.is_const) { err.set("probe_block: column dtype/length mismatch (const probe columns unsupported)"); return DBX_ERR_INVALID; }
       DBX_TRY(stager.stage(col, c, &cols[c]));
     }
-    int64_t out_cap = n + n / 8 + 1024;  // optimistic: about one match per probe row
+    // RIGHT SEMI / RIGHT ANTI only mark the matched map here: no output columns, no blocks
+    const bool marks_only = prm.kind == DBX_JOIN_RIGHT_SEMI || prm.kind == DBX_JOIN_RIGHT_ANTI;
+    int64_t out_cap = marks_only ? 0 : n + n / 8 + 1024;  // optimistic: about one match per probe row
     DBX_TRY(timing_begin());
     // radix probe: reorder the block region by region (row order of a join result is unspecified)
     bool can_part = n_part > 1 && (n >= (1 << 16) || getenv("DBX_JOIN_REGION_BYTES"));
@@ -645,12 +728,13 @@ class JoinOp : public Op {
       memset(&pp, 0, sizeof(pp));
       pp.key = cols[prm.probe_key_col];
       pp.table = table_view();
-      pp.n_probe_cols = n_probe_cols;
-      pp.n_build_cols = (prm.kind == DBX_JOIN_INNER || prm.kind == DBX_JOIN_LEFT) ? n_build_cols : 0;
+      pp.n_probe_cols = marks_only ? 0 : n_probe_cols;
+      pp.n_build_cols = (prm.kind == DBX_JOIN_INNER || prm.kind == DBX_JOIN_LEFT || prm.kind == DBX_JOIN_RIGHT || prm.kind == DBX_JOIN_FULL) ? n_build_cols : 0;
       pp.kind = prm.kind;
       pp.n_rows = n;
       pp.out_cap = out_cap;
       pp.cursor = (unsigned long long*)cursor.p;
+      pp.matched = build_side_kind(prm.kind) ? (uint8_t*)matched.p : nullptr;
       std::vector<uint8_t*> valid_bytes;
       auto add_out = [&](JoinColDev& jc, int dtype, bool nullable) -> int32_t {
         void* d = nullptr;
@@ -671,12 +755,14 @@ class JoinOp : public Op {
         ob->cols.push_back(oc);
         return DBX_OK;
       };
-      // output column order = probe projection then build projection (inner_join.rs:236-245)
-      for (int c = 0; c < n_probe_cols; ++c) {
+      // output column order = probe projection then build projection (inner_join.rs:236-245);
+      // RIGHT and FULL return the probe columns Nullable in every block (their final blocks carry NULLs there)
+      const bool probe_null = prm.kind == DBX_JOIN_RIGHT || prm.kind == DBX_JOIN_FULL;
+      for (int c = 0; c < pp.n_probe_cols; ++c) {
         pp.probe_cols[c].src = cols[c].data;
         pp.probe_cols[c].src_validity = cols[c].validity;
         pp.probe_cols[c].src_vbit_off = cols[c].vbit_off;
-        DBX_TRY(add_out(pp.probe_cols[c], probe_dtype[c], probe_nullable[c]));
+        DBX_TRY(add_out(pp.probe_cols[c], probe_dtype[c], probe_nullable[c] || probe_null));
       }
       DevBuf build_bits[kMaxJoinCols];
       for (int c = 0; c < pp.n_build_cols; ++c) {
@@ -688,7 +774,7 @@ class JoinOp : public Op {
           count_launch();
           pp.build_cols[c].src_validity = (const uint8_t*)build_bits[c].p;
         }
-        DBX_TRY(add_out(pp.build_cols[c], build_dtype[c], build_nullable[c] || prm.kind == DBX_JOIN_LEFT));
+        DBX_TRY(add_out(pp.build_cols[c], build_dtype[c], build_nullable[c] || prm.kind == DBX_JOIN_LEFT || prm.kind == DBX_JOIN_FULL));
       }
       DBX_CUDA_TRY(err, cudaMemsetAsync(cursor.p, 0, 8, stream));
       if (can_part) {  // region by region: stream the region into L2, then probe the rows that hash into it
@@ -735,6 +821,86 @@ class JoinOp : public Op {
     return DBX_OK;
   }
 
+  // Join::final_probe (right_join.rs, right_join_semi.rs, right_join_anti.rs; FULL as in
+  // hash_join_probe_state.rs:455-567): once every probe block is done, queue the build rows that were
+  // never matched (RIGHT, RIGHT ANTI, FULL) or matched at least once (RIGHT SEMI), for dbx_op_pull.
+  // RIGHT and FULL put Const NULL entries on the probe side (the reference's null_block), so
+  // nothing is written for them.  A no-op for the probe-side kinds, and for a second call.
+  int32_t final_probe() {
+    if (!finished) { err.set("final_probe before final_build"); return DBX_ERR_STATE; }
+    if (final_probed) return DBX_OK;
+    final_probed = true;
+    if (!build_side_kind(prm.kind) || build_rows == 0) return DBX_OK;
+    JoinFinalParams fp;
+    memset(&fp, 0, sizeof(fp));
+    fp.n_cols = n_build_cols;
+    fp.want = prm.kind == DBX_JOIN_RIGHT_SEMI ? 1 : 0;
+    fp.matched = (const uint8_t*)matched.p;
+    fp.n_rows = build_rows;
+    fp.cursor = (unsigned long long*)cursor.p;
+    // pass 1 counts (out_cap = 0), so the output is allocated exactly
+    DBX_TRY(timing_begin());
+    DBX_CUDA_TRY(err, cudaMemsetAsync(cursor.p, 0, 8, stream));
+    join_final_scan_kernel<<<grid_rows(build_rows), kJoinBlock, 0, stream>>>(fp);
+    count_launch();
+    DBX_CUDA_TRY(err, cudaGetLastError());
+    DBX_TRY(timing_end());
+    DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, cursor.p, 8, cudaMemcpyDeviceToHost, stream));
+    DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
+    const int64_t rows = (int64_t)*(unsigned long long*)host.p;
+    if (rows == 0) return DBX_OK;
+    auto ob = std::make_unique<OwnedBlock>();
+    ob->stream = stream;
+    ob->device = device;
+    if (prm.kind == DBX_JOIN_RIGHT || prm.kind == DBX_JOIN_FULL) {
+      for (int c = 0; c < n_probe_cols; ++c) {
+        dbx_column oc;
+        memset(&oc, 0, sizeof(oc));
+        oc.dtype = probe_dtype[c]; oc.mem = DBX_MEM_DEVICE; oc.is_const = 1; oc.len = rows; oc.null_count = rows;
+        oc.konst.dtype = probe_dtype[c]; oc.konst.is_null = 1;
+        ob->cols.push_back(oc);
+      }
+    }
+    std::vector<uint8_t*> valid_bytes;
+    for (int c = 0; c < n_build_cols; ++c) {
+      const int sz = build[c].size;
+      void* d = nullptr;
+      DBX_CUDA_TRY(err, pool_alloc(device, stream, (size_t)rows * sz, &d));
+      ob->dev_allocs.push_back(d);
+      uint8_t* vb = nullptr;
+      if (build_nullable[c] || prm.kind == DBX_JOIN_FULL) {
+        DBX_CUDA_TRY(err, pool_alloc(device, stream, (size_t)rows, (void**)&vb));
+        ob->dev_allocs.push_back(vb);
+      }
+      valid_bytes.push_back(vb);
+      fp.cols[c] = FinalColDev{build[c].data.p, build[c].nullable ? (const uint8_t*)build[c].valid_bytes.p : nullptr, d, vb, sz, 0};
+      dbx_column oc;
+      memset(&oc, 0, sizeof(oc));
+      oc.dtype = build_dtype[c]; oc.mem = DBX_MEM_DEVICE; oc.data = d; oc.len = rows; oc.null_count = vb ? -1 : 0;
+      ob->cols.push_back(oc);
+    }
+    fp.out_cap = rows;
+    DBX_TRY(timing_begin());
+    DBX_CUDA_TRY(err, cudaMemsetAsync(cursor.p, 0, 8, stream));
+    join_final_scan_kernel<<<grid_rows(build_rows), kJoinBlock, 0, stream>>>(fp);
+    count_launch();
+    DBX_CUDA_TRY(err, cudaGetLastError());
+    DBX_TRY(timing_end());
+    const size_t first_build = ob->cols.size() - (size_t)n_build_cols;
+    for (int c = 0; c < n_build_cols; ++c) {
+      if (!valid_bytes[c]) continue;
+      uint8_t* bits = nullptr;
+      DBX_CUDA_TRY(err, pool_alloc(device, stream, (size_t)(rows + 7) / 8 + 8, (void**)&bits));
+      ob->dev_allocs.push_back(bits);
+      pack_bits_kernel<<<grid_rows((rows + 7) / 8 + 1), kJoinBlock, 0, stream>>>(valid_bytes[c], rows, bits);
+      count_launch();
+      ob->cols[first_build + c].validity = bits;
+    }
+    DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
+    outputs.push_back(std::move(ob));
+    return DBX_OK;
+  }
+
   // JoinStream::next
   int32_t pull(int32_t out_mem, dbx_block* out, int32_t* has_block) override {
     if (next_out >= outputs.size()) { *has_block = 0; outputs.clear(); next_out = 0; return DBX_OK; }
@@ -746,6 +912,7 @@ class JoinOp : public Op {
     for (const dbx_column& dc : ob->cols) {
       dbx_column c = dc;
       c.mem = DBX_MEM_HOST;
+      if (dc.is_const) { hb->cols.push_back(c); continue; }  // Const entries carry no data
       size_t bytes = (size_t)dc.len * dtype_size(dc.dtype);
       void* hp = nullptr;
       DBX_CUDA_TRY(err, pinned_alloc(bytes, &hp));
@@ -768,6 +935,7 @@ class JoinOp : public Op {
 
   int32_t reset() override {
     build_rows = 0;
+    final_probed = false;  // the matched map is cleared by the next final_build
     outputs.clear();
     next_out = 0;
     return DBX_OK;
@@ -791,4 +959,12 @@ extern "C" int32_t dbx_join_probe(dbx_op* op, const dbx_block* block) {
   if (o->kind != DBX_OP_JOIN) { o->err.set("dbx_join_probe: not a join operator"); return DBX_ERR_INVALID; }
   DBX_CUDA_TRY(o->err, cudaSetDevice(o->device));
   return static_cast<JoinOp*>(o)->probe(block);
+}
+
+extern "C" int32_t dbx_join_final_probe(dbx_op* op) {
+  if (!op) return DBX_ERR_INVALID;
+  Op* o = reinterpret_cast<Op*>(op);
+  if (o->kind != DBX_OP_JOIN) { o->err.set("dbx_join_final_probe: not a join operator"); return DBX_ERR_INVALID; }
+  DBX_CUDA_TRY(o->err, cudaSetDevice(o->device));
+  return static_cast<JoinOp*>(o)->final_probe();
 }

@@ -72,16 +72,18 @@ def shuffle_by_key(block: DataBlock, key_col: int, device: int, group=None) -> T
 
 
 def partitioned_hash_join(build: DataBlock, probe: DataBlock, build_key: int, probe_key: int, device: int, group=None,
-                          out_mem: int = abi.MEM_HOST):
-    """Inner join of two row-range-sharded tables: shuffle both sides by key, then join locally.
-    Returns the joined blocks of this rank (probe columns then build columns)."""
+                          out_mem: int = abi.MEM_HOST, kind: int = abi.JOIN_INNER):
+    """Join of two row-range-sharded tables: shuffle both sides by key, then join locally.
+    Returns the joined blocks of this rank (probe columns then build columns).  Each rank owns
+    every build row of its keys, so its final_probe stream (the build-side kinds) is complete."""
     b_local, keep_b = shuffle_by_key(build, build_key, device, group)
     p_local, keep_p = shuffle_by_key(probe, probe_key, device, group)
     torch.cuda.synchronize(device)
-    j = HashJoin(schema_types(b_local), schema_types(p_local), build_key, probe_key, device)
+    j = HashJoin(schema_types(b_local), schema_types(p_local), build_key, probe_key, device, kind)
     j.add_block(b_local)
     j.final_build()
     out = j.probe_block(p_local, out_mem)
+    out += j.final_probe(out_mem)
     return out, j, (keep_b, keep_p)
 
 
@@ -229,6 +231,11 @@ class PartitionedHashJoin:
         outs = []
         for m in self._rounds(self.sp, probe, self.max_probe, lambda b: outs.extend(j.probe_block(b, out_mem)), j, ms):
             ms["probe"] += m
+        # Join::final_probe after the last round: this rank owns every build row of its keys, so its
+        # matched map is complete (a no-op for INNER and the LEFT kinds)
+        t0 = time.perf_counter()
+        outs.extend(j.final_probe(out_mem))
+        ms["final_probe"] = (time.perf_counter() - t0) * 1e3
         if stats is not None:
             stats.update(ms)
         return outs, j

@@ -60,6 +60,7 @@ def load():
         "dbx_op_reset": (i32, [vp]),
         "dbx_op_synchronize": (i32, [vp]),
         "dbx_join_probe": (i32, [vp, P(abi.Block)]),
+        "dbx_join_final_probe": (i32, [vp]),
         "dbx_agg_final_merge_partial": (i32, [vp, vp]),
         "dbx_agg_partial_partition": (i32, [vp, i32, P(vp), P(i64), P(i32)]),
         "dbx_agg_final_merge_rows": (i32, [vp, vp, i64]),

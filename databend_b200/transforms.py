@@ -335,15 +335,20 @@ class TransformTopN(_Op):
 
 
 class HashJoin(_Op):
-    """Inner hash join behind the reference's `Join` trait (new_hash_join/join.rs:26-53):
-    add_block(build block) / final_build() / probe_block(block) -> joined blocks.
+    """Hash join behind the reference's `Join` trait (new_hash_join/join.rs:26-53):
+    add_block(build block) / final_build() / probe_block(block) -> joined blocks /
+    final_probe() -> the build rows a build-side join keeps.
     Output columns = probe columns then build columns (inner_join.rs:236-245); output row order is
     unspecified (compare as multisets)."""
 
     def __init__(self, build_types: Sequence[int], probe_types: Sequence[int], build_key: int, probe_key: int,
                  device: int = 0, kind: int = abi.JOIN_INNER, expected_build_rows: int = 0):
-        """kind: abi.JOIN_INNER, JOIN_LEFT_SEMI or JOIN_LEFT_ANTI (probe side = left; semi/anti
-        emit probe columns only: left_join_semi.rs / left_join_anti.rs)."""
+        """kind (probe side = left, build side = right):
+          JOIN_INNER, JOIN_LEFT (probe rows kept), JOIN_LEFT_SEMI / JOIN_LEFT_ANTI (probe columns only:
+          left_join_semi.rs / left_join_anti.rs);
+          JOIN_RIGHT (build rows kept: final_probe emits the unmatched ones with NULL probe columns),
+          JOIN_RIGHT_SEMI / JOIN_RIGHT_ANTI (build columns only, all from final_probe), JOIN_FULL
+          (LEFT during the probe, then RIGHT's final stream)."""
         p = abi.JoinParams()
         p.kind, p.build_key_col, p.probe_key_col, p.n_build_cols = kind, build_key, probe_key, len(build_types)
         p.expected_build_rows = expected_build_rows
@@ -358,6 +363,19 @@ class HashJoin(_Op):
     def probe_block(self, block: DataBlock, out_mem: int = abi.MEM_HOST) -> List[DataBlock]:
         b, keep = block.as_c()
         check(load().dbx_join_probe(self._h, C.byref(b)), self._h)
+        out = []
+        while True:
+            ob = self.pull_c(out_mem)
+            if ob is None:
+                break
+            out.append(_block_from_c(ob, self.device) if out_mem == abi.MEM_HOST else ob)
+        return out
+
+    def final_probe(self, out_mem: int = abi.MEM_HOST) -> List[DataBlock]:
+        """Join::final_probe, called once after the last probe_block: the build rows that RIGHT,
+        RIGHT ANTI and FULL keep unmatched, or that RIGHT SEMI matched (each once).  Empty for the
+        other kinds and on a second call.  probe_block fails after it until reset()."""
+        check(load().dbx_join_final_probe(self._h), self._h)
         out = []
         while True:
             ob = self.pull_c(out_mem)

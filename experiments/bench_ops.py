@@ -26,6 +26,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--ops", default="join,topk,sort,filter,eval")
 ap.add_argument("--sort-rows", type=int, default=250_000_000)
 ap.add_argument("--join-shuffle", default="peer", choices=["peer", "nccl"])
+ap.add_argument("--join-kind", default="inner", choices=["inner", "left", "right", "right_semi", "right_anti", "full"])
 ap.add_argument("--round-rows", type=int, default=32 << 20)
 ap.add_argument("--fact-rows", type=int, default=1_000_000_000)
 ap.add_argument("--dim-rows", type=int, default=10_000_000)
@@ -74,14 +75,22 @@ def emit(d):
 ops = a.ops.split(",")
 
 if "join" in ops:
-    # configs[2]: fact(fk uniform over the dim keys, fv) JOIN dim(dk = 0..D-1 hashed anyway, dv); every fact row matches once
+    # configs[2]: fact(fk uniform over the dim keys, fv) JOIN dim(dk = 0..D-1 hashed anyway, dv); every fact row matches once.
+    # The other kinds use a second dim variant: every 10th dim key is moved out of the facts' range
+    # (dk = i + D for i % 10 == 9), so 10 % of the dim rows are never matched (RIGHT / RIGHT ANTI /
+    # FULL have a final stream) and 10 % of the fact rows find no dim row.
+    join_kind = {"inner": abi.JOIN_INNER, "left": abi.JOIN_LEFT, "right": abi.JOIN_RIGHT, "right_semi": abi.JOIN_RIGHT_SEMI,
+                 "right_anti": abi.JOIN_RIGHT_ANTI, "full": abi.JOIN_FULL}[a.join_kind]
     F, D = a.fact_rows, a.dim_rows
     f0, f1 = F * rank // world, F * (rank + 1) // world
     d0, d1 = D * rank // world, D * (rank + 1) // world
     nf, nd = f1 - f0, d1 - d0
     fk, fv = fill(0, 7, D, f0, nf), fill(1, 8, 0, f0, nf)
     dk = DeviceBuffer(max(1, nd * 8), dev)
-    dk.upload(np.arange(d0, d1, dtype=np.int64))
+    dkeys = np.arange(d0, d1, dtype=np.int64)
+    if join_kind != abi.JOIN_INNER:
+        dkeys[dkeys % 10 == 9] += D
+    dk.upload(dkeys)
     dv = fill(1, 9, 0, d0, nd)
     dim = DataBlock([Column.device(abi.I64, nd, dk.ptr), Column.device(abi.I64, nd, dv.ptr)], nd)
     fact = DataBlock([Column.device(abi.I64, nf, fk.ptr), Column.device(abi.I64, nf, fv.ptr)], nf)
@@ -92,7 +101,7 @@ if "join" in ops:
         from databend_b200.distributed import PartitionedHashJoin
         mx = torch.tensor([nd, nf], dtype=torch.int64, device=f"cuda:{dev}")
         dist.all_reduce(mx, op=dist.ReduceOp.MAX)
-        pj = PartitionedHashJoin([abi.I64, abi.I64], [abi.I64, abi.I64], 0, 0, dev, rank, world, int(mx[0]), int(mx[1]), a.round_rows)
+        pj = PartitionedHashJoin([abi.I64, abi.I64], [abi.I64, abi.I64], 0, 0, dev, rank, world, int(mx[0]), int(mx[1]), a.round_rows, kind=join_kind)
     for rep in range(a.reps):
         sync_all()
         t0 = time.perf_counter()
@@ -108,7 +117,7 @@ if "join" in ops:
             total = time.perf_counter() - t0
             j.close()
             rec = (max_over_ranks(total), max_over_ranks((st["shuffle_send"] + st["shuffle_wait"]) * 1e-3), max_over_ranks(st["build"] * 1e-3),
-                   max_over_ranks(st["probe"] * 1e-3), max_over_ranks(st["probe"]), out_rows)
+                   max_over_ranks(st["probe"] * 1e-3), max_over_ranks(st["probe"]), out_rows, max_over_ranks(st["final_probe"]))
             if best is None or rec[0] < best[0]:
                 best = rec
                 best_stats = {k_: max_over_ranks(v_) for k_, v_ in st.items()}
@@ -122,7 +131,7 @@ if "join" in ops:
         else:
             dim_l, fact_l = dim, fact
         t_shuffle = time.perf_counter() - t0
-        j = HashJoin([abi.I64, abi.I64], [abi.I64, abi.I64], 0, 0, dev)
+        j = HashJoin([abi.I64, abi.I64], [abi.I64, abi.I64], 0, 0, dev, join_kind)
         tb = time.perf_counter()
         j.add_block(dim_l)
         j.final_build()
@@ -137,23 +146,38 @@ if "join" in ops:
             for ob in outs:
                 out_rows += ob.num_rows
                 L.dbx_block_release(C.byref(ob))
+        # Join::final_probe (build-side kinds): a counting pass over the matched map, then, when rows
+        # are selected, the compacting pass; both are timed with events (kernel_ms(0) is the last)
+        final_ms = 0.0
+        if join_kind >= abi.JOIN_RIGHT:
+            fouts = j.final_probe(abi.MEM_DEVICE)
+            final_ms = j.kernel_ms(0) + (j.kernel_ms(1) if fouts else 0.0)
+            for ob in fouts:
+                out_rows += ob.num_rows
+                L.dbx_block_release(C.byref(ob))
         j.synchronize()
         t_probe = time.perf_counter() - tp
         sync_all()
         total = time.perf_counter() - t0
         j.close()
         del keep
-        rec = (max_over_ranks(total), max_over_ranks(t_shuffle), max_over_ranks(t_build), max_over_ranks(t_probe), max_over_ranks(probe_ms), out_rows)
+        rec = (max_over_ranks(total), max_over_ranks(t_shuffle), max_over_ranks(t_build), max_over_ranks(t_probe), max_over_ranks(probe_ms), out_rows,
+               max_over_ranks(final_ms))
         if best is None or rec[0] < best[0]:
             best = rec
     if pj is not None:
         pj.close()
-    total, t_shuffle, t_build, t_probe, probe_ms, out_rows = best
+    total, t_shuffle, t_build, t_probe, probe_ms, out_rows, final_ms = best
     ot = torch.tensor([out_rows], dtype=torch.int64, device=f"cuda:{dev}")
     if world > 1:
         dist.all_reduce(ot)
     rows_per_gpu = F / world
-    emit({"op": "hash_join", "workload": "configs[2]: fact 1e9 x dim 1e7 inner join on int64 key, (fk, fv, dk, dv) materialised", "n_gpus": world,
+    kind_fields = {} if join_kind == abi.JOIN_INNER else {
+        "join_kind": a.join_kind, "final_probe_ms": final_ms,
+        "dim_variant": "every 10th dim key moved out of the facts' range: 10 % of dim rows unmatched, 10 % of fact rows without a dim row",
+        "final_probe_timing": "multi-GPU: host wall clock of final_probe per rank" if world > 1 and a.join_shuffle == "peer" else
+                              "CUDA events: counting pass + compacting pass of the final scan (probe_kernel_ms covers the probe blocks only)"}
+    emit({"op": "hash_join", "workload": "configs[2]: fact 1e9 x dim 1e7 inner join on int64 key, (fk, fv, dk, dv) materialised", "n_gpus": world, **kind_fields,
           "fact_rows": F, "dim_rows": D, "joined_rows": int(ot.item()), "rows_per_s": F / total, "total_ms": total * 1e3,
           "shuffle_ms": t_shuffle * 1e3, "build_ms": t_build * 1e3, "probe_wall_ms": t_probe * 1e3, "probe_kernel_ms": probe_ms,
           "roofline": {"bound": "hbm", "bytes_per_fact_row": 64, "note": "read fk,fv (16) + table bucket (32-byte sector) + write 4 x 8 (32) = 80 with dk materialised; 56 by SURVEY 8d (3 output columns, dim row gather)",

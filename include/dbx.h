@@ -211,8 +211,21 @@ typedef struct dbx_topk_params {
  * probe columns only (left_join_semi.rs, left_join_anti.rs; a NULL probe key never matches, so
  * ANTI keeps the row).
  * LEFT (outer, probe side preserved; left_join.rs): every probe row; rows without a match carry
- * NULL in all build columns, which therefore come back Nullable.  Output row order is unspecified. */
-typedef enum dbx_join_kind { DBX_JOIN_INNER = 0, DBX_JOIN_LEFT_SEMI = 1, DBX_JOIN_LEFT_ANTI = 2, DBX_JOIN_LEFT = 3 } dbx_join_kind;
+ * NULL in all build columns, which therefore come back Nullable.
+ * The build-side ("right") kinds keep build rows.  Matches accumulate over all probe blocks and
+ * dbx_join_final_probe then emits the build rows (a build row with a NULL key never matches):
+ *   RIGHT (right_join.rs): probe blocks emit every match as INNER; final_probe emits every build
+ *     row never matched, with NULL probe columns.  Probe columns come back Nullable in every block.
+ *   RIGHT_SEMI / RIGHT_ANTI (right_join_semi.rs, right_join_anti.rs): probe blocks emit nothing;
+ *     final_probe emits each build row matched at least once / never matched, build columns only.
+ *   FULL (hash_join_probe_state.rs:455-567): probe blocks as LEFT, final_probe as RIGHT; every
+ *     column comes back Nullable.
+ * The NULL probe side of a final block is a Const NULL entry (is_const = 1, konst.is_null = 1).
+ * Output row order is unspecified. */
+typedef enum dbx_join_kind {
+  DBX_JOIN_INNER = 0, DBX_JOIN_LEFT_SEMI = 1, DBX_JOIN_LEFT_ANTI = 2, DBX_JOIN_LEFT = 3,
+  DBX_JOIN_RIGHT = 4, DBX_JOIN_RIGHT_SEMI = 5, DBX_JOIN_RIGHT_ANTI = 6, DBX_JOIN_FULL = 7
+} dbx_join_kind;
 typedef struct dbx_join_params {
   int32_t kind;          /* dbx_join_kind */
   int32_t build_key_col; /* key column index in build blocks */
@@ -281,8 +294,13 @@ int32_t dbx_op_synchronize(dbx_op* op);
 int32_t dbx_op_inputs_consumed(dbx_op* op);
 
 /* Join probe side: Join::probe_block(block) -> JoinStream::next()* ; output blocks are
- * pulled with dbx_op_pull until drained.  Join::final_probe is a no-op for inner joins. */
+ * pulled with dbx_op_pull until drained. */
 int32_t dbx_join_probe(dbx_op* op, const dbx_block* block);
+/* Join::final_probe -> JoinStream::next()* : after the last probe block, queue the build rows the
+ * build-side kinds emit (see dbx_join_kind); pull them with dbx_op_pull until drained.  Queues
+ * nothing for INNER and the LEFT kinds, and nothing on a second call.  dbx_join_probe after it
+ * returns DBX_ERR_STATE until dbx_op_reset. */
+int32_t dbx_join_final_probe(dbx_op* op);
 
 /* AGG_FINAL input: hand over a partial operator's device-resident payload
  * (AggregateMeta::AggregatePayload, aggregate_meta.rs) without leaving HBM. */

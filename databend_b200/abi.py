@@ -127,6 +127,9 @@ class TopkParams(C.Structure):
     ]
 
 
+MAX_JOIN_KEYS = 4
+
+
 class JoinParams(C.Structure):
     _fields_ = [
         ("kind", C.c_int32),
@@ -134,6 +137,9 @@ class JoinParams(C.Structure):
         ("probe_key_col", C.c_int32),
         ("n_build_cols", C.c_int32),
         ("expected_build_rows", C.c_int64),
+        ("n_extra_keys", C.c_int32),
+        ("extra_build_key_cols", C.c_int32 * (MAX_JOIN_KEYS - 1)),
+        ("extra_probe_key_cols", C.c_int32 * (MAX_JOIN_KEYS - 1)),
     ]
 
 

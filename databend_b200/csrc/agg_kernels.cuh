@@ -307,9 +307,7 @@ __device__ __noinline__ int64_t find_or_insert_slow(const TableDev& t, uint64_t 
 // ---- 128-bit packed keys: slot i holds keys[2 i], keys[2 i + 1]; a bucket is 2 slots = one 32-byte
 // sector = one 256-bit probe; insertion is ONE 128-bit compare-and-swap (atom.cas.b128, sm_90+).
 // The EMPTY pattern is both words == kEmptyKey; a real key equal to it lives in the special slot cap.
-__device__ __forceinline__ uint64_t agg_hash_wide(uint64_t k0, uint64_t k1) {
-  return agg_hash_u64(k0 ^ (agg_hash_u64(k1) + 0x9e3779b97f4a7c15ULL));
-}
+// (agg_hash_wide is in common.cuh: the join hashes its 128-bit keys with it too.)
 __device__ __forceinline__ void cas_b128(uint64_t* addr, uint64_t c0, uint64_t c1, uint64_t v0, uint64_t v1, uint64_t& o0, uint64_t& o1) {
   asm volatile(
       "{\n\t"

@@ -194,6 +194,10 @@ __host__ __device__ __forceinline__ uint64_t agg_hash_u64(uint64_t x) {
   return x;
 }
 constexpr uint64_t kNullHashVal = 0xd1cefa08eb382d69ULL;  // group_hash.rs:38
+// 128-bit packed keys (multi-column GROUP BY and join keys wider than 64 bits)
+__device__ __forceinline__ uint64_t agg_hash_wide(uint64_t k0, uint64_t k1) {
+  return agg_hash_u64(k0 ^ (agg_hash_u64(k1) + 0x9e3779b97f4a7c15ULL));
+}
 
 // Owner / partition of a hash among n parts: the top 32 hash bits scaled to [0, n), i.e.
 // mulhi32(hash >> 32, n) — radix partitioning on the top bits (partitioned_payload.rs:44-57)

@@ -21,10 +21,18 @@
 // take_column_vec).  Output row order is therefore unspecified — like the reference's when
 // several threads build the chains — and results are compared as multisets.
 // NULL keys never match (fixed_keys.rs: rows with a NULL key are skipped on both sides).
+//
+// Composite keys (up to four key pairs, HashMethodFixedKeys in new_hash_join/hashtable/fixed_keys.rs)
+// are packed into one or two 64-bit words, one bit field per pair (KeyPartDev, as the aggregate's
+// multi-column GROUP BY).  Up to 64 bits the entry is the same as for one key; up to 128 bits it is
+// {k0, k1, row1, p0}: still one sector, with one inlined build column instead of two.  The kernels
+// are templated on the key width KW (words) and on PACKED (key loaded from several columns); the
+// single-key instantiations <1, false> are the code as it was before composite keys.
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
 
+#include "plan.h"
 #include "runtime.h"
 
 namespace dbx {
@@ -34,12 +42,40 @@ namespace {
 constexpr int kJoinBlock = 256;
 constexpr int kMaxJoinCols = 16;
 
-struct JoinEntry {
+template <int KW> struct JEntry;
+template <> struct JEntry<1> {
   uint64_t key;
   uint64_t row1;  // (build row + 1) | validity of p0 << 62 | validity of p1 << 63; 0 = empty
   uint64_t p0, p1;  // raw bytes of up to two build columns (zero-extended to 8 bytes)
 };
+template <> struct JEntry<2> {  // 128-bit key
+  uint64_t key, key1;
+  uint64_t row1;  // (build row + 1) | validity of p0 << 62; 0 = empty
+  uint64_t p0;
+};
+using JoinEntry = JEntry<1>;
+static_assert(sizeof(JEntry<1>) == 32 && sizeof(JEntry<2>) == 32, "one entry = one 32-byte sector");
 constexpr uint64_t kRowMask = (1ULL << 62) - 1;
+
+__device__ __forceinline__ void clear_entry(JEntry<1>& e) { e.key = e.row1 = e.p0 = e.p1 = 0; }
+__device__ __forceinline__ void clear_entry(JEntry<2>& e) { e.key = e.key1 = e.row1 = e.p0 = 0; }
+__device__ __forceinline__ bool key_eq(const JEntry<1>& e, uint64_t k, uint64_t) { return e.key == k; }
+__device__ __forceinline__ bool key_eq(const JEntry<2>& e, uint64_t k, uint64_t kh) { return e.key == k && e.key1 == kh; }
+__device__ __forceinline__ uint64_t key_hi(const JEntry<1>&) { return 0; }
+__device__ __forceinline__ uint64_t key_hi(const JEntry<2>& e) { return e.key1; }
+__device__ __forceinline__ uint64_t entry_p1(const JEntry<1>& e) { return e.p1; }
+__device__ __forceinline__ uint64_t entry_p1(const JEntry<2>&) { return 0; }
+__device__ __forceinline__ void fill_entry(JEntry<1>* e, uint64_t k, uint64_t, uint64_t p0, uint64_t p1) { e->key = k; e->p0 = p0; e->p1 = p1; }
+__device__ __forceinline__ void fill_entry(JEntry<2>* e, uint64_t k, uint64_t kh, uint64_t p0, uint64_t) { e->key = k; e->key1 = kh; e->p0 = p0; }
+
+// Composite key of one side: its key columns and the bit field of each (KeyPartDev: shift, mask,
+// dtype; slot = column index).  Both sides share shifts and masks and differ in dtypes.
+struct JoinKeyPack {
+  DevCol cols[DBX_MAX_JOIN_KEYS];
+  KeyPartDev parts[DBX_MAX_JOIN_KEYS];
+  int32_t n;
+  int32_t pad;
+};
 
 // Radix layout: the table is cut into n_part regions of `region` entries (both powers of two);
 // a key lives in region part_owner(key, n_part) (top hash bits) at slot hash & (region - 1)
@@ -53,8 +89,9 @@ struct JoinTableDev {
   int32_t n_part;
   int32_t pad;
 };
-__device__ __forceinline__ int64_t join_home(const JoinTableDev& t, uint64_t k, int64_t* region_base) {
-  const uint64_t h = agg_hash_u64(k);
+template <int KW = 1>
+__device__ __forceinline__ int64_t join_home(const JoinTableDev& t, uint64_t k, int64_t* region_base, uint64_t kh = 0) {
+  const uint64_t h = KW == 1 ? agg_hash_u64(k) : agg_hash_wide(k, kh);
   const int64_t part = t.n_part > 1 ? (int64_t)hash_to_part(h, t.n_part) : 0;
   *region_base = part * t.region;
   return (int64_t)(h & (uint64_t)(t.region - 1));
@@ -76,7 +113,8 @@ struct JoinColDev {
   int64_t src_vbit_off;
   uint8_t* dst_valid;           // one byte per output row, or null
   int32_t size;                 // bytes per value
-  int32_t from;                 // build side: 0 gather by build row, 1 the entry's key, 2 entry.p0, 3 entry.p1
+  int32_t from;                 // build side: 0 gather by build row, 1 the entry's key, 2 entry.p0, 3 entry.p1,
+                                // 4 + s: the packed key's bit field at shift s (composite keys)
 };
 
 struct JoinProbeParams {
@@ -91,6 +129,7 @@ struct JoinProbeParams {
   int64_t out_cap;
   unsigned long long* cursor;  // number of matches (may exceed out_cap: then the host retries)
   uint8_t* matched;            // build-side kinds: one byte per build row, set when a probe row matches it
+  JoinKeyPack pack;            // composite keys (PACKED kernels): the probe key columns
 };
 
 __device__ __forceinline__ uint64_t load_key(const DevCol& c, int64_t row) {
@@ -117,23 +156,48 @@ __device__ __forceinline__ uint64_t load_raw(const void* base, int size, int64_t
     default: return ((const uint8_t*)base)[row];
   }
 }
+// Composite key of row r: false if any key column is NULL there (the row never matches).  Each
+// value is widened to 64 bits (load_key), masked to its field and shifted into word shift / 64.
+template <int KW>
+__device__ __forceinline__ bool load_packed_key(const JoinKeyPack& pk, int64_t r, uint64_t& k, uint64_t& kh) {
+  k = kh = 0;
+#pragma unroll
+  for (int i = 0; i < DBX_MAX_JOIN_KEYS; ++i) {
+    if (i >= pk.n) break;
+    const DevCol& c = pk.cols[i];
+    if (c.validity && !bit_test(c.validity, c.vbit_off + r)) return false;
+    const KeyPartDev& f = pk.parts[i];
+    const uint64_t v = (load_key(c, r) & f.mask) << (f.shift & 63);
+    if (KW == 1 || f.shift < 64) k |= v;
+    else kh |= v;
+  }
+  return true;
+}
+
+template <int KW, bool PACKED>
 __global__ void join_build_kernel(const __grid_constant__ DevCol key, int64_t n_rows, int64_t row_base,
                                   const __grid_constant__ JoinTableDev t, const __grid_constant__ InlineColDev i0,
-                                  const __grid_constant__ InlineColDev i1) {
+                                  const __grid_constant__ InlineColDev i1, const __grid_constant__ JoinKeyPack pk) {
   const int64_t mask = t.region - 1;
+  JEntry<KW>* const entries = (JEntry<KW>*)t.entries;
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
-    if (key.validity && !bit_test(key.validity, key.vbit_off + r)) continue;
-    const uint64_t k = load_key(key, r);
+    uint64_t k, kh = 0;
+    if (PACKED) {
+      if (!load_packed_key<KW>(pk, r, k, kh)) continue;
+    } else {
+      if (key.validity && !bit_test(key.validity, key.vbit_off + r)) continue;
+      k = load_key(key, r);
+    }
     uint64_t tag = (uint64_t)(row_base + r + 1);
     uint64_t p0 = 0, p1 = 0;
     if (i0.on) { p0 = load_raw(i0.src, i0.size, r); if (!i0.valid_bytes || i0.valid_bytes[r]) tag |= 1ULL << 62; }
-    if (i1.on) { p1 = load_raw(i1.src, i1.size, r); if (!i1.valid_bytes || i1.valid_bytes[r]) tag |= 1ULL << 63; }
+    if (KW == 1 && i1.on) { p1 = load_raw(i1.src, i1.size, r); if (!i1.valid_bytes || i1.valid_bytes[r]) tag |= 1ULL << 63; }
     int64_t rb;
-    int64_t s = join_home(t, k, &rb);
+    int64_t s = join_home<KW>(t, k, &rb, kh);
     for (;;) {
-      JoinEntry* e = t.entries + rb + s;
+      JEntry<KW>* e = entries + rb + s;
       unsigned long long old = atomicCAS((unsigned long long*)&e->row1, 0ULL, (unsigned long long)tag);
-      if (old == 0ULL) { e->key = k; e->p0 = p0; e->p1 = p1; break; }
+      if (old == 0ULL) { fill_entry(e, k, kh, p0, p1); break; }
       s = (s + 1) & mask;
     }
   }
@@ -173,7 +237,18 @@ __device__ __forceinline__ JoinEntry load_entry(const JoinEntry* e) {
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.p0), "=l"(r.p1) : "l"((const char*)e + 16), "l"(pol));
   return r;
 }
-__device__ __forceinline__ void emit_match(const JoinProbeParams& p, int64_t r, const JoinEntry& e, int64_t pos) {
+__device__ __forceinline__ JEntry<2> load_entry(const JEntry<2>* e) {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  JEntry<2> r;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.key), "=l"(r.key1) : "l"(e), "l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;" : "=l"(r.row1), "=l"(r.p0) : "l"((const char*)e + 16), "l"(pol));
+  return r;
+}
+// PACKED: the build key columns are decoded from the entry's packed key (from = 4 + field shift),
+// which saves the random gather by build row that a key column would otherwise cost.
+template <bool PACKED = false, int KW>
+__device__ __forceinline__ void emit_match(const JoinProbeParams& p, int64_t r, const JEntry<KW>& e, int64_t pos) {
   if (pos >= p.out_cap) return;
   for (int c = 0; c < p.n_probe_cols; ++c) copy_value(p.probe_cols[c], r, pos);
   for (int c = 0; c < p.n_build_cols; ++c) {
@@ -181,7 +256,11 @@ __device__ __forceinline__ void emit_match(const JoinProbeParams& p, int64_t r, 
     if (jc.from == 0) copy_value(jc, (int64_t)(e.row1 & kRowMask) - 1, pos);
     else if (jc.from == 1) store_value(jc, e.key, true, pos);
     else if (jc.from == 2) store_value(jc, e.p0, (e.row1 >> 62) & 1, pos);
-    else store_value(jc, e.p1, (e.row1 >> 63) & 1, pos);
+    else if (!PACKED || jc.from == 3) store_value(jc, entry_p1(e), (e.row1 >> 63) & 1, pos);
+    else {
+      const int s = jc.from - 4;
+      store_value(jc, (s < 64 ? e.key : key_hi(e)) >> (s & 63), true, pos);
+    }
   }
 }
 __global__ void __launch_bounds__(kJoinBlock) join_probe_kernel(const __grid_constant__ JoinProbeParams p) {
@@ -260,17 +339,19 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe_kernel(const __grid_con
 // probe sequence (short at load factor <= 0.5).  A build side without duplicates (the usual
 // primary-key dimension table) lets the probe stop at its first match instead of walking on to the
 // next empty entry: one dependent L2 round trip per probe row instead of two or more.
+template <int KW>
 __global__ void join_dup_check_kernel(const __grid_constant__ JoinTableDev t, unsigned int* dup) {
   const int64_t mask = t.region - 1;
+  const JEntry<KW>* const entries = (const JEntry<KW>*)t.entries;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < t.cap; i += (int64_t)gridDim.x * blockDim.x) {
-    const JoinEntry e = t.entries[i];
+    const JEntry<KW> e = entries[i];
     if (e.row1 == 0) continue;
     const int64_t rb = i & ~mask;
     int64_t s = (i + 1) & mask;
     for (;;) {
-      const JoinEntry f = t.entries[rb + s];
+      const JEntry<KW> f = entries[rb + s];
       if (f.row1 == 0) break;
-      if (f.key == e.key) { *dup = 1; break; }
+      if (key_eq(f, e.key, key_hi(e))) { *dup = 1; break; }
       s = (s + 1) & mask;
       if (rb + s == i) break;
     }
@@ -283,8 +364,12 @@ __global__ void join_dup_check_kernel(const __grid_constant__ JoinTableDev t, un
 // MARK (the build-side kinds RIGHT, RIGHT SEMI, RIGHT ANTI, FULL): every matching entry's build
 // row is marked in p.matched for the final scan.  Racing stores all write 1, so no atomics.  RIGHT
 // then emits like INNER, FULL like LEFT, RIGHT SEMI / ANTI emit nothing here.
-template <bool UNIQUE, bool MARK>
-__global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
+// KW / PACKED: key width in words and composite keys (see the top of the file); a probe row with a
+// NULL in any key column is a miss.  The PACKED instantiations ask for three resident blocks per
+// SM: without a minimum ptxas caps them near 64 registers and spills, with one it takes up to 94
+// registers (two blocks per SM), and the probe is bound by latency, so occupancy counts.
+template <int KW, bool PACKED, bool UNIQUE, bool MARK>
+__global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
   __shared__ unsigned int s_warp[kJoinBlock / 32];
   __shared__ unsigned long long s_base;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -292,36 +377,38 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_co
   const int64_t step = (int64_t)gridDim.x * blockDim.x * 2;
   const int64_t n_iter = (p.n_rows + step - 1) / step;
   const int64_t row_end = p.row_begin + p.n_rows;
+  const JEntry<KW>* const entries = (const JEntry<KW>*)p.table.entries;
   for (int64_t it = 0; it < n_iter; ++it) {
     int64_t r[2];
     r[0] = p.row_begin + it * step + (int64_t)blockIdx.x * blockDim.x * 2 + threadIdx.x;
     r[1] = r[0] + blockDim.x;
     bool in_range[2], go[2];
-    uint64_t k[2] = {0, 0};
+    uint64_t k[2] = {0, 0}, kh[2] = {0, 0};
     int64_t b0[2] = {0, 0}, rb[2] = {0, 0}, sl[2] = {0, 0};
     unsigned int n_match[2] = {0, 0};
-    JoinEntry first[2];
+    JEntry<KW> first[2];
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
-      first[j].key = first[j].row1 = first[j].p0 = first[j].p1 = 0;
+      clear_entry(first[j]);
       in_range[j] = r[j] < row_end;
-      go[j] = in_range[j] && !(p.key.validity && !bit_test(p.key.validity, p.key.vbit_off + r[j]));
+      if (PACKED) go[j] = in_range[j] && load_packed_key<KW>(p.pack, r[j], k[j], kh[j]);
+      else go[j] = in_range[j] && !(p.key.validity && !bit_test(p.key.validity, p.key.vbit_off + r[j]));
       if (go[j]) {
-        k[j] = load_key(p.key, r[j]);
-        b0[j] = join_home(p.table, k[j], &rb[j]);
+        if (!PACKED) k[j] = load_key(p.key, r[j]);
+        b0[j] = join_home<KW>(p.table, k[j], &rb[j], kh[j]);
         sl[j] = b0[j];
       }
     }
     while (go[0] || go[1]) {  // an empty entry ends a probe sequence
-      JoinEntry e[2];
+      JEntry<KW> e[2];
 #pragma unroll
       for (int j = 0; j < 2; ++j)
-        if (go[j]) e[j] = load_entry(p.table.entries + rb[j] + sl[j]);
+        if (go[j]) e[j] = load_entry(entries + rb[j] + sl[j]);
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         if (!go[j]) continue;
         if (e[j].row1 == 0) { go[j] = false; continue; }
-        if (e[j].key == k[j]) {
+        if (key_eq(e[j], k[j], kh[j])) {
           if (MARK) {  // read first: a dimension row hit by many facts is written once, not per match
             uint8_t* m = p.matched + (int64_t)(e[j].row1 & kRowMask) - 1;
             if (*m == 0) *m = 1;
@@ -374,14 +461,14 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe2_kernel(const __grid_co
           for (int c = 0; c < p.n_probe_cols; ++c) copy_value(p.probe_cols[c], r[j], pos);
         ++pos;
       } else if (n_match[j]) {
-        emit_match(p, r[j], first[j], pos++);
+        emit_match<PACKED>(p, r[j], first[j], pos++);
         if (!UNIQUE && n_match[j] > 1) {  // duplicates of the key on the build side: walk again, skip the first
           int64_t b = b0[j];
           unsigned int seen = 0;
           for (;;) {
-            const JoinEntry e = load_entry(p.table.entries + rb[j] + b);
+            const JEntry<KW> e = load_entry(entries + rb[j] + b);
             if (e.row1 == 0) break;
-            if (e.key == k[j] && seen++ > 0) emit_match(p, r[j], e, pos++);
+            if (key_eq(e, k[j], kh[j]) && seen++ > 0) emit_match<PACKED>(p, r[j], e, pos++);
             b = (b + 1) & mask;
           }
         }
@@ -515,6 +602,16 @@ class JoinOp : public Op {
   size_t next_out = 0;
   DevBuf matched;             // build-side kinds: one byte per build row, 1 once any probe row matched it
   bool final_probed = false;  // Join::final_probe ran: no more probe blocks until reset
+  // key pairs (1 + n_extra_keys); packed: composite key of key_words words, fields in *_part
+  int n_keys = 1, key_words = 1;
+  bool packed = false;
+  int key_build_col[DBX_MAX_JOIN_KEYS], key_probe_col[DBX_MAX_JOIN_KEYS];
+  KeyPartDev build_part[DBX_MAX_JOIN_KEYS], probe_part[DBX_MAX_JOIN_KEYS];
+  // bit field of build column c in the packed key, -1 if c is not a key column
+  int build_key_shift(int c) const {
+    for (int i = 0; i < n_keys; ++i) if (key_build_col[i] == c) return build_part[i].shift;
+    return -1;
+  }
 
   // input_types = build schema (params.n_build_cols columns) followed by the probe schema.
   int32_t init(const dbx_join_params* p, const int32_t* types, int32_t n, int dev) {
@@ -530,8 +627,16 @@ class JoinOp : public Op {
     for (int i = 0; i < n_build_cols; ++i) { build_dtype[i] = types[i] & 0xFF; build_nullable[i] = (types[i] & DBX_NULLABLE) != 0; }
     for (int i = 0; i < n_probe_cols; ++i) { probe_dtype[i] = types[n_build_cols + i] & 0xFF; probe_nullable[i] = (types[n_build_cols + i] & DBX_NULLABLE) != 0; }
     if (p->build_key_col < 0 || p->build_key_col >= n_build_cols || p->probe_key_col < 0 || p->probe_key_col >= n_probe_cols) { err.set("join: key column outside the schema"); return DBX_ERR_INVALID; }
+    if (p->n_extra_keys < 0 || p->n_extra_keys > DBX_MAX_JOIN_KEYS - 1) { err.set("join: n_extra_keys must be 0 .. DBX_MAX_JOIN_KEYS - 1"); return DBX_ERR_INVALID; }
+    n_keys = 1 + p->n_extra_keys;
+    for (int i = 0; i < n_keys; ++i) {
+      key_build_col[i] = i == 0 ? p->build_key_col : p->extra_build_key_cols[i - 1];
+      key_probe_col[i] = i == 0 ? p->probe_key_col : p->extra_probe_key_cols[i - 1];
+      if (key_build_col[i] < 0 || key_build_col[i] >= n_build_cols || key_probe_col[i] < 0 || key_probe_col[i] >= n_probe_cols) { err.set("join: key column outside the schema"); return DBX_ERR_INVALID; }
+    }
     auto int_key = [](int dt) { return dt != DBX_BOOL && dt != DBX_F32 && dt != DBX_F64 && dtype_size(dt) > 0; };
-    if (!int_key(build_dtype[p->build_key_col]) || !int_key(probe_dtype[p->probe_key_col])) { err.set("join: keys must be integer columns"); return DBX_ERR_UNSUPPORTED; }
+    for (int i = 0; i < n_keys; ++i)
+      if (!int_key(build_dtype[key_build_col[i]]) || !int_key(probe_dtype[key_probe_col[i]])) { err.set("join: keys must be integer columns"); return DBX_ERR_UNSUPPORTED; }
     for (int i = 0; i < n_build_cols; ++i) if (dtype_size(build_dtype[i]) == 0) { err.set("join: only fixed-width numeric columns are supported"); return DBX_ERR_UNSUPPORTED; }
     for (int i = 0; i < n_probe_cols; ++i) if (dtype_size(probe_dtype[i]) == 0) { err.set("join: only fixed-width numeric columns are supported"); return DBX_ERR_UNSUPPORTED; }
     // keys of different widths/signedness compare by value: both are widened to 64 bits
@@ -539,10 +644,37 @@ class JoinOp : public Op {
     // with no 64-bit super type is (signed, UInt64): the widened images of -1 and 2^64-1 coincide,
     // so it is refused here (the reference's type checker casts both sides to a wider type first;
     // a caller wanting that join casts the keys before the operator, as the reference's planner does).
-    {
-      const int bk = build_dtype[p->build_key_col], pk = probe_dtype[p->probe_key_col];
+    for (int i = 0; i < n_keys; ++i) {
+      const int bk = build_dtype[key_build_col[i]], pk = probe_dtype[key_probe_col[i]];
       const bool bs = dtype_class(bk) == VC_INT, ps = dtype_class(pk) == VC_INT;
       if ((bk == DBX_U64 && ps) || (pk == DBX_U64 && bs)) { err.set("join: a signed key cannot be compared with a UInt64 key without a cast (no common 64-bit type)"); return DBX_ERR_UNSUPPORTED; }
+    }
+    // composite keys: one bit field per pair, as wide as the pair's common type (same signedness:
+    // the larger size; signed S with unsigned U: max(S, 2U) bytes, which holds both value ranges),
+    // packed from bit 0 upward; a field never straddles the two words (the aggregate's rule)
+    packed = n_keys > 1;
+    key_words = 1;
+    if (packed) {
+      int bits = 0;
+      for (int i = 0; i < n_keys; ++i) {
+        const int bk = build_dtype[key_build_col[i]], pk = probe_dtype[key_probe_col[i]];
+        const int bsz = dtype_size(bk), psz = dtype_size(pk);
+        const bool bs = dtype_class(bk) == VC_INT, ps = dtype_class(pk) == VC_INT;
+        const int bytes = bs == ps ? std::max(bsz, psz) : (bs ? std::max(bsz, 2 * psz) : std::max(psz, 2 * bsz));
+        const int w = 8 * bytes;
+        if (bits < 64 && bits + w > 64) bits = 64;
+        for (KeyPartDev* kp : {&build_part[i], &probe_part[i]}) {
+          memset(kp, 0, sizeof(*kp));
+          kp->shift = bits;
+          kp->null_shift = -1;  // NULL rows never enter the table or match: no NULL flags
+          kp->mask = w == 64 ? ~0ULL : ((1ULL << w) - 1);
+        }
+        build_part[i].slot = key_build_col[i]; build_part[i].dtype = bk;
+        probe_part[i].slot = key_probe_col[i]; probe_part[i].dtype = pk;
+        bits += w;
+      }
+      if (bits > 128) { err.set("join: composite keys wider than 128 bits need 256-bit or serialised join keys: not built"); return DBX_ERR_UNSUPPORTED; }
+      key_words = bits > 64 ? 2 : 1;
     }
     build.resize(n_build_cols);
     for (int i = 0; i < n_build_cols; ++i) { build[i].size = dtype_size(build_dtype[i]); build[i].nullable = build_nullable[i]; }
@@ -602,9 +734,10 @@ class JoinOp : public Op {
       // Radix regions are OFF by default: once the probe stops at its first match (unique build
       // keys) one random HBM sector per row costs less than the extra partition pass over the
       // probe block.  DBX_JOIN_REGION_BYTES=<bytes> turns them on (tests exercise both).
+      // Composite keys stay in one region: hash_partition_device partitions by one column.
       int64_t target = 0;
       if (const char* e = getenv("DBX_JOIN_REGION_BYTES")) target = atoll(e);
-      if (target > 0 && bytes > 3 * target) {
+      if (!packed && target > 0 && bytes > 3 * target) {
         while (n_part < kMaxParts && bytes / n_part > target) n_part *= 2;
       }
     }
@@ -636,19 +769,39 @@ class JoinOp : public Op {
       key.dtype = build_dtype[prm.build_key_col];
       // build-side validity is stored as bytes; expose it as a bitmap-free predicate by packing
       DevBuf kbits;
-      if (kc.nullable) {
+      if (kc.nullable && !packed) {
         DBX_CUDA_TRY(err, kbits.ensure((size_t)(build_rows + 7) / 8 + 8));
         pack_bits_kernel<<<grid_rows((build_rows + 7) / 8), kJoinBlock, 0, stream>>>((const uint8_t*)kc.valid_bytes.p, build_rows, (uint8_t*)kbits.p);
         count_launch();
         key.validity = (const uint8_t*)kbits.p;
       }
+      // composite keys: every key column, NULL bitmaps packed from the stored bytes as above
+      JoinKeyPack pk;
+      memset(&pk, 0, sizeof(pk));
+      DevBuf pk_bits[DBX_MAX_JOIN_KEYS];
+      if (packed) {
+        pk.n = n_keys;
+        for (int i = 0; i < n_keys; ++i) {
+          const GrowCol& g = build[key_build_col[i]];
+          pk.cols[i].data = g.data.p;
+          pk.cols[i].dtype = build_dtype[key_build_col[i]];
+          pk.parts[i] = build_part[i];
+          if (g.nullable) {
+            DBX_CUDA_TRY(err, pk_bits[i].ensure((size_t)(build_rows + 7) / 8 + 8));
+            pack_bits_kernel<<<grid_rows((build_rows + 7) / 8), kJoinBlock, 0, stream>>>((const uint8_t*)g.valid_bytes.p, build_rows, (uint8_t*)pk_bits[i].p);
+            count_launch();
+            pk.cols[i].validity = (const uint8_t*)pk_bits[i].p;
+          }
+        }
+      }
       JoinTableDev t = table_view();
-      // the first two non-key build columns travel inside the entries
+      // the first two non-key build columns travel inside the entries (one with a 128-bit key)
       InlineColDev ic[2];
       memset(ic, 0, sizeof(ic));
       inline_col[0] = inline_col[1] = -1;
-      for (int c = 0, k = 0; c < n_build_cols && k < 2; ++c) {
-        if (c == prm.build_key_col) continue;
+      const int n_inline = key_words == 2 ? 1 : 2;
+      for (int c = 0, k = 0; c < n_build_cols && k < n_inline; ++c) {
+        if (packed ? build_key_shift(c) >= 0 : c == prm.build_key_col) continue;
         inline_col[k] = c;
         ic[k].src = build[c].data.p;
         ic[k].valid_bytes = build[c].nullable ? (const uint8_t*)build[c].valid_bytes.p : nullptr;
@@ -656,11 +809,15 @@ class JoinOp : public Op {
         ic[k].on = 1;
         ++k;
       }
-      join_build_kernel<<<grid_rows(build_rows), kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1]);
+      const int grid = grid_rows(build_rows);
+      if (!packed) join_build_kernel<1, false><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1], pk);
+      else if (key_words == 1) join_build_kernel<1, true><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1], pk);
+      else join_build_kernel<2, true><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1], pk);
       count_launch();
       DBX_CUDA_TRY(err, cudaGetLastError());
       DBX_CUDA_TRY(err, cudaMemsetAsync(cursor.p, 0, 16, stream));
-      join_dup_check_kernel<<<grid_rows(table_cap), kJoinBlock, 0, stream>>>(t, (unsigned int*)cursor.p + 2);
+      if (key_words == 2) join_dup_check_kernel<2><<<grid_rows(table_cap), kJoinBlock, 0, stream>>>(t, (unsigned int*)cursor.p + 2);
+      else join_dup_check_kernel<1><<<grid_rows(table_cap), kJoinBlock, 0, stream>>>(t, (unsigned int*)cursor.p + 2);
       count_launch();
       DBX_CUDA_TRY(err, cudaGetLastError());
       DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, (unsigned int*)cursor.p + 2, 4, cudaMemcpyDeviceToHost, stream));
@@ -672,17 +829,28 @@ class JoinOp : public Op {
     return DBX_OK;
   }
 
+  template <int KW, bool PACKED>
+  void launch_probe2(const JoinProbeParams& pp, int grid) {
+    if (pp.matched) {
+      if (build_unique) join_probe2_kernel<KW, PACKED, true, true><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<KW, PACKED, false, true><<<grid, kJoinBlock, 0, stream>>>(pp);
+    } else {
+      if (build_unique) join_probe2_kernel<KW, PACKED, true, false><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<KW, PACKED, false, false><<<grid, kJoinBlock, 0, stream>>>(pp);
+    }
+  }
   void launch_probe(const JoinProbeParams& pp, int64_t rows) {
     static const bool old_probe = getenv("DBX_JOIN_OLD_PROBE") != nullptr;
     const int grid = grid_rows((rows + 1) / 2);
-    if (pp.matched) {  // build-side kinds: always the two-row kernel (DBX_JOIN_OLD_PROBE is an ablation of the probe-side kinds)
-      if (build_unique) join_probe2_kernel<true, true><<<grid, kJoinBlock, 0, stream>>>(pp);
-      else join_probe2_kernel<false, true><<<grid, kJoinBlock, 0, stream>>>(pp);
+    // DBX_JOIN_OLD_PROBE is an ablation of the single-key probe-side kinds; the build-side kinds and
+    // composite keys always take the two-row kernel
+    if (packed) {
+      if (key_words == 2) launch_probe2<2, true>(pp, grid);
+      else launch_probe2<1, true>(pp, grid);
       return;
     }
-    if (old_probe) { join_probe_kernel<<<grid_rows(rows), kJoinBlock, 0, stream>>>(pp); return; }
-    if (build_unique) join_probe2_kernel<true, false><<<grid, kJoinBlock, 0, stream>>>(pp);
-    else join_probe2_kernel<false, false><<<grid, kJoinBlock, 0, stream>>>(pp);
+    if (old_probe && !pp.matched) { join_probe_kernel<<<grid_rows(rows), kJoinBlock, 0, stream>>>(pp); return; }
+    launch_probe2<1, false>(pp, grid);
   }
 
   // Join::probe_block: join one probe block; the joined block is queued for dbx_op_pull
@@ -735,6 +903,13 @@ class JoinOp : public Op {
       pp.out_cap = out_cap;
       pp.cursor = (unsigned long long*)cursor.p;
       pp.matched = build_side_kind(prm.kind) ? (uint8_t*)matched.p : nullptr;
+      if (packed) {
+        pp.pack.n = n_keys;
+        for (int i = 0; i < n_keys; ++i) {
+          pp.pack.cols[i] = cols[key_probe_col[i]];
+          pp.pack.parts[i] = probe_part[i];
+        }
+      }
       std::vector<uint8_t*> valid_bytes;
       auto add_out = [&](JoinColDev& jc, int dtype, bool nullable) -> int32_t {
         void* d = nullptr;
@@ -767,7 +942,8 @@ class JoinOp : public Op {
       DevBuf build_bits[kMaxJoinCols];
       for (int c = 0; c < pp.n_build_cols; ++c) {
         pp.build_cols[c].src = build[c].data.p;
-        pp.build_cols[c].from = c == prm.build_key_col ? 1 : (c == inline_col[0] ? 2 : (c == inline_col[1] ? 3 : 0));
+        if (packed && build_key_shift(c) >= 0) pp.build_cols[c].from = 4 + build_key_shift(c);  // decoded from the entry's key
+        else pp.build_cols[c].from = c == prm.build_key_col ? 1 : (c == inline_col[0] ? 2 : (c == inline_col[1] ? 3 : 0));
         if (build[c].nullable && pp.build_cols[c].from == 0) {  // bytes -> use the byte array directly through a 1-byte "bitmap" trick: pack once
           DBX_CUDA_TRY(err, build_bits[c].ensure((size_t)(build_rows + 7) / 8 + 8));
           pack_bits_kernel<<<grid_rows((build_rows + 7) / 8), kJoinBlock, 0, stream>>>((const uint8_t*)build[c].valid_bytes.p, build_rows, (uint8_t*)build_bits[c].p);

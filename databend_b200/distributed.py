@@ -71,13 +71,21 @@ def shuffle_by_key(block: DataBlock, key_col: int, device: int, group=None) -> T
     return DataBlock(cols, n), recv
 
 
-def partitioned_hash_join(build: DataBlock, probe: DataBlock, build_key: int, probe_key: int, device: int, group=None,
+def _first_key(key) -> int:
+    return int(key) if isinstance(key, (int, np.integer)) else int(key[0])
+
+
+def partitioned_hash_join(build: DataBlock, probe: DataBlock, build_key, probe_key, device: int, group=None,
                           out_mem: int = abi.MEM_HOST, kind: int = abi.JOIN_INNER):
     """Join of two row-range-sharded tables: shuffle both sides by key, then join locally.
     Returns the joined blocks of this rank (probe columns then build columns).  Each rank owns
-    every build row of its keys, so its final_probe stream (the build-side kinds) is complete."""
-    b_local, keep_b = shuffle_by_key(build, build_key, device, group)
-    p_local, keep_p = shuffle_by_key(probe, probe_key, device, group)
+    every build row of its keys, so its final_probe stream (the build-side kinds) is complete.
+    build_key / probe_key: a column index or equally long lists (composite keys, see HashJoin).
+    Both sides are shuffled on the FIRST key pair only: rows equal on every key are equal on the
+    first, and both sides hash the same 64-bit image of it.  A first key with few distinct values
+    therefore puts most rows on few ranks."""
+    b_local, keep_b = shuffle_by_key(build, _first_key(build_key), device, group)
+    p_local, keep_p = shuffle_by_key(probe, _first_key(probe_key), device, group)
     torch.cuda.synchronize(device)
     j = HashJoin(schema_types(b_local), schema_types(p_local), build_key, probe_key, device, kind)
     j.add_block(b_local)
@@ -183,16 +191,18 @@ class PartitionedHashJoin:
     rank and round; every received region is handed to the local join as a device block.
     Reference: flight_scatter_hash.rs:86-125 (scatter) + new_hash_join/memory/inner_join.rs:122-262.
     The constructor is collective (receive buffers + IPC mapping, once per schema); `run` joins one
-    pair of row-range-sharded tables."""
+    pair of row-range-sharded tables.  Composite keys (lists of column indices, see HashJoin) are
+    shuffled on their first pair, as in partitioned_hash_join: a low-cardinality first key skews
+    the ranks."""
 
-    def __init__(self, build_types: Sequence[int], probe_types: Sequence[int], build_key: int, probe_key: int, device: int, rank: int,
+    def __init__(self, build_types: Sequence[int], probe_types: Sequence[int], build_key, probe_key, device: int, rank: int,
                  world: int, max_build_rows: int, max_probe_rows: int, round_rows: int = 32 << 20, group=None, kind: int = abi.JOIN_INNER):
         from .exchange import PeerShuffle
         self.device, self.rank, self.world, self.round_rows = device, rank, world, round_rows
         self.build_types, self.probe_types, self.build_key, self.probe_key, self.kind = list(build_types), list(probe_types), build_key, probe_key, kind
         self.max_build, self.max_probe = max_build_rows, max_probe_rows
-        self.sb = PeerShuffle(device, rank, world, [t & 0xFF for t in build_types], build_key, max(1, min(round_rows, max_build_rows)))
-        self.sp = PeerShuffle(device, rank, world, [t & 0xFF for t in probe_types], probe_key, max(1, min(round_rows, max_probe_rows)))
+        self.sb = PeerShuffle(device, rank, world, [t & 0xFF for t in build_types], _first_key(build_key), max(1, min(round_rows, max_build_rows)))
+        self.sp = PeerShuffle(device, rank, world, [t & 0xFF for t in probe_types], _first_key(probe_key), max(1, min(round_rows, max_probe_rows)))
         if world > 1:
             self.sb.connect(group)
             self.sp.connect(group)
@@ -245,7 +255,7 @@ class PartitionedHashJoin:
         self.sp.close()
 
 
-def partitioned_hash_join_peer(build: DataBlock, probe: DataBlock, build_key: int, probe_key: int, device: int, rank: int, world: int,
+def partitioned_hash_join_peer(build: DataBlock, probe: DataBlock, build_key, probe_key, device: int, rank: int, world: int,
                                round_rows: int = 32 << 20, out_mem: int = abi.MEM_HOST, group=None, kind: int = abi.JOIN_INNER,
                                stats: dict = None):
     """One-shot form of PartitionedHashJoin (set-up included): returns (joined blocks, join op, [the object to close])."""

@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass, field
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -334,6 +334,35 @@ class TransformTopN(_Op):
         return _block_from_c(b, self.device)
 
 
+def _key_list(key) -> List[int]:
+    return [int(key)] if isinstance(key, (int, np.integer)) else [int(k) for k in key]
+
+
+_SIGNED = (abi.I8, abi.I16, abi.I32, abi.I64)
+_KEY_BYTES = {abi.I8: 1, abi.U8: 1, abi.I16: 2, abi.U16: 2, abi.I32: 4, abi.U32: 4, abi.I64: 8, abi.U64: 8}
+
+
+def join_key_layout(build_dtypes: Sequence[int], probe_dtypes: Sequence[int]) -> Tuple[List[Tuple[int, int]], int]:
+    """The composite join key's bit fields as the operator packs them: [(shift, width in bits)] per key
+    pair and the total bits, with a field never straddling bit 64.  A pair's width is its common
+    type's: the larger size for equal signedness, max(S, 2 U) bytes for signed S with unsigned U.
+    Up to 64 bits the table key is one word, up to 128 bits two; wider layouts are refused."""
+    fields, bits = [], 0
+    for b, p in zip(build_dtypes, probe_dtypes):
+        b, p = b & 0xFF, p & 0xFF
+        if b not in _KEY_BYTES or p not in _KEY_BYTES:
+            raise DbxError(abi.ERR_UNSUPPORTED, "join: keys must be integer columns")
+        bs, ps, bz, pz = b in _SIGNED, p in _SIGNED, _KEY_BYTES[b], _KEY_BYTES[p]
+        if (b == abi.U64 and ps) or (p == abi.U64 and bs):
+            raise DbxError(abi.ERR_UNSUPPORTED, "join: a signed key cannot be compared with a UInt64 key without a cast")
+        w = 8 * (max(bz, pz) if bs == ps else max(bz, 2 * pz) if bs else max(pz, 2 * bz))
+        if bits < 64 < bits + w:
+            bits = 64
+        fields.append((bits, w))
+        bits += w
+    return fields, bits
+
+
 class HashJoin(_Op):
     """Hash join behind the reference's `Join` trait (new_hash_join/join.rs:26-53):
     add_block(build block) / final_build() / probe_block(block) -> joined blocks /
@@ -341,17 +370,26 @@ class HashJoin(_Op):
     Output columns = probe columns then build columns (inner_join.rs:236-245); output row order is
     unspecified (compare as multisets)."""
 
-    def __init__(self, build_types: Sequence[int], probe_types: Sequence[int], build_key: int, probe_key: int,
-                 device: int = 0, kind: int = abi.JOIN_INNER, expected_build_rows: int = 0):
+    def __init__(self, build_types: Sequence[int], probe_types: Sequence[int], build_key: Union[int, Sequence[int]],
+                 probe_key: Union[int, Sequence[int]], device: int = 0, kind: int = abi.JOIN_INNER, expected_build_rows: int = 0):
         """kind (probe side = left, build side = right):
           JOIN_INNER, JOIN_LEFT (probe rows kept), JOIN_LEFT_SEMI / JOIN_LEFT_ANTI (probe columns only:
           left_join_semi.rs / left_join_anti.rs);
           JOIN_RIGHT (build rows kept: final_probe emits the unmatched ones with NULL probe columns),
           JOIN_RIGHT_SEMI / JOIN_RIGHT_ANTI (build columns only, all from final_probe), JOIN_FULL
-          (LEFT during the probe, then RIGHT's final stream)."""
+          (LEFT during the probe, then RIGHT's final stream).
+        build_key / probe_key: one column index each, or equally long sequences of up to
+        abi.MAX_JOIN_KEYS indices (ON b[0] = p[0] AND b[1] = p[1] ...; a NULL in any key column never
+        matches).  The keys are packed into 64 or 128 bits (join_key_layout)."""
+        bkeys, pkeys = _key_list(build_key), _key_list(probe_key)
+        if len(bkeys) != len(pkeys) or not 1 <= len(bkeys) <= abi.MAX_JOIN_KEYS:
+            raise DbxError(abi.ERR_INVALID, f"join: build and probe keys must be 1 .. {abi.MAX_JOIN_KEYS} columns each, as many on both sides")
         p = abi.JoinParams()
-        p.kind, p.build_key_col, p.probe_key_col, p.n_build_cols = kind, build_key, probe_key, len(build_types)
+        p.kind, p.build_key_col, p.probe_key_col, p.n_build_cols = kind, bkeys[0], pkeys[0], len(build_types)
         p.expected_build_rows = expected_build_rows
+        p.n_extra_keys = len(bkeys) - 1
+        for i in range(1, len(bkeys)):
+            p.extra_build_key_cols[i - 1], p.extra_probe_key_cols[i - 1] = bkeys[i], pkeys[i]
         super().__init__(abi.OP_JOIN, p, list(build_types) + list(probe_types), device)
 
     def add_block(self, block: DataBlock):

@@ -18,7 +18,7 @@ import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
 from databend_b200 import abi, expr as E  # noqa: E402
-from databend_b200.block import Column, DataBlock  # noqa: E402
+from databend_b200.block import Column, DataBlock, np_dtype  # noqa: E402
 from databend_b200.lib import check, load  # noqa: E402
 from databend_b200.transforms import DeviceBuffer, HashJoin, TransformFilter, TransformTopN  # noqa: E402
 
@@ -27,6 +27,9 @@ ap.add_argument("--ops", default="join,topk,sort,filter,eval")
 ap.add_argument("--sort-rows", type=int, default=250_000_000)
 ap.add_argument("--join-shuffle", default="peer", choices=["peer", "nccl"])
 ap.add_argument("--join-kind", default="inner", choices=["inner", "left", "right", "right_semi", "right_anti", "full"])
+# key layout of the join (the same unique key either way): one Int64 column; split into two Int32
+# columns (lo, hi; the 64-bit packed key); or two Int64 columns (k, -k; the 128-bit packed key)
+ap.add_argument("--join-keys", default="i64", choices=["i64", "2xi32", "2xi64"])
 ap.add_argument("--round-rows", type=int, default=32 << 20)
 ap.add_argument("--fact-rows", type=int, default=1_000_000_000)
 ap.add_argument("--dim-rows", type=int, default=10_000_000)
@@ -92,8 +95,28 @@ if "join" in ops:
         dkeys[dkeys % 10 == 9] += D
     dk.upload(dkeys)
     dv = fill(1, 9, 0, d0, nd)
-    dim = DataBlock([Column.device(abi.I64, nd, dk.ptr), Column.device(abi.I64, nd, dv.ptr)], nd)
-    fact = DataBlock([Column.device(abi.I64, nf, fk.ptr), Column.device(abi.I64, nf, fv.ptr)], nf)
+    key_hold = []  # device tensors behind the derived key columns
+
+    def key_cols(buf, n):
+        """the join key columns of one side in the --join-keys layout (the first one is unique: the shuffle key)"""
+        if a.join_keys == "i64":
+            return [Column.device(abi.I64, n, buf.ptr)]
+        from databend_b200.distributed import _dev_tensor
+        k = _dev_tensor(buf.ptr, n * 8, dev).view(torch.int64)
+        if a.join_keys == "2xi32":
+            parts, dt = [(k & 0xFFFFFFFF).to(torch.int32), (k >> 32).to(torch.int32)], abi.I32
+        else:
+            parts, dt = [k.clone(), -k], abi.I64
+        key_hold.extend(parts)
+        return [Column.device(dt, n, t.data_ptr()) for t in parts]
+    dim_keys, fact_keys = key_cols(dk, nd), key_cols(fk, nf)
+    torch.cuda.synchronize(dev)
+    n_keys = len(dim_keys)
+    key_ids = list(range(n_keys)) if n_keys > 1 else 0
+    side_types = [c.dtype for c in dim_keys] + [abi.I64]
+    key_bytes = sum(np_dtype(c.dtype).itemsize for c in fact_keys)
+    dim = DataBlock(dim_keys + [Column.device(abi.I64, nd, dv.ptr)], nd)
+    fact = DataBlock(fact_keys + [Column.device(abi.I64, nf, fv.ptr)], nf)
     best = None
     best_stats = None
     pj = None
@@ -101,7 +124,7 @@ if "join" in ops:
         from databend_b200.distributed import PartitionedHashJoin
         mx = torch.tensor([nd, nf], dtype=torch.int64, device=f"cuda:{dev}")
         dist.all_reduce(mx, op=dist.ReduceOp.MAX)
-        pj = PartitionedHashJoin([abi.I64, abi.I64], [abi.I64, abi.I64], 0, 0, dev, rank, world, int(mx[0]), int(mx[1]), a.round_rows, kind=join_kind)
+        pj = PartitionedHashJoin(side_types, side_types, key_ids, key_ids, dev, rank, world, int(mx[0]), int(mx[1]), a.round_rows, kind=join_kind)
     for rep in range(a.reps):
         sync_all()
         t0 = time.perf_counter()
@@ -131,7 +154,7 @@ if "join" in ops:
         else:
             dim_l, fact_l = dim, fact
         t_shuffle = time.perf_counter() - t0
-        j = HashJoin([abi.I64, abi.I64], [abi.I64, abi.I64], 0, 0, dev, join_kind)
+        j = HashJoin(side_types, side_types, key_ids, key_ids, dev, join_kind)
         tb = time.perf_counter()
         j.add_block(dim_l)
         j.final_build()
@@ -177,7 +200,11 @@ if "join" in ops:
         "dim_variant": "every 10th dim key moved out of the facts' range: 10 % of dim rows unmatched, 10 % of fact rows without a dim row",
         "final_probe_timing": "multi-GPU: host wall clock of final_probe per rank" if world > 1 and a.join_shuffle == "peer" else
                               "CUDA events: counting pass + compacting pass of the final scan (probe_kernel_ms covers the probe blocks only)"}
-    emit({"op": "hash_join", "workload": "configs[2]: fact 1e9 x dim 1e7 inner join on int64 key, (fk, fv, dk, dv) materialised", "n_gpus": world, **kind_fields,
+    key_fields = {} if a.join_keys == "i64" else {
+        "join_keys": a.join_keys, "key_bytes_per_fact_row": key_bytes,
+        "key_layout": "two Int32 columns (lo, hi) of the unique key: 64-bit packed key" if a.join_keys == "2xi32" else
+                      "two Int64 columns (k, -k): 128-bit packed key, one inlined build column"}
+    emit({"op": "hash_join", "workload": "configs[2]: fact 1e9 x dim 1e7 inner join on int64 key, (fk, fv, dk, dv) materialised", "n_gpus": world, **kind_fields, **key_fields,
           "fact_rows": F, "dim_rows": D, "joined_rows": int(ot.item()), "rows_per_s": F / total, "total_ms": total * 1e3,
           "shuffle_ms": t_shuffle * 1e3, "build_ms": t_build * 1e3, "probe_wall_ms": t_probe * 1e3, "probe_kernel_ms": probe_ms,
           "roofline": {"bound": "hbm", "bytes_per_fact_row": 64, "note": "read fk,fv (16) + table bucket (32-byte sector) + write 4 x 8 (32) = 80 with dk materialised; 56 by SURVEY 8d (3 output columns, dim row gather)",

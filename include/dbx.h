@@ -221,7 +221,19 @@ typedef struct dbx_topk_params {
  *   FULL (hash_join_probe_state.rs:455-567): probe blocks as LEFT, final_probe as RIGHT; every
  *     column comes back Nullable.
  * The NULL probe side of a final block is a Const NULL entry (is_const = 1, konst.is_null = 1).
- * Output row order is unspecified. */
+ * Output row order is unspecified.
+ *
+ * Composite keys (n_extra_keys > 0): ON build_key_col = probe_key_col AND extra_build_key_cols[i]
+ * = extra_probe_key_cols[i] ... (up to DBX_MAX_JOIN_KEYS pairs; the fixed_keys.rs idea).  A row with
+ * a NULL in ANY key column never matches, on either side.  Keys compare by value: each pair becomes
+ * one bit field as wide as the pair's common type (same signedness: the larger size; signed S with
+ * unsigned U: max(S, 2 U) bytes), each value sign- or zero-extended to the field and masked.  Fields
+ * are packed from bit 0 upward and never straddle bit 64.  Up to 64 bits the table key is one word,
+ * up to 128 bits two words; wider keys (256-bit or serialised join keys) are not built and are
+ * refused with DBX_ERR_UNSUPPORTED, as are float / bool keys and a signed key paired with a UInt64
+ * one (no common 64-bit type, also for a single key).  n_extra_keys outside 0 .. DBX_MAX_JOIN_KEYS - 1
+ * or a key column outside its schema: DBX_ERR_INVALID.  A zeroed tail is the single-key join. */
+#define DBX_MAX_JOIN_KEYS 4
 typedef enum dbx_join_kind {
   DBX_JOIN_INNER = 0, DBX_JOIN_LEFT_SEMI = 1, DBX_JOIN_LEFT_ANTI = 2, DBX_JOIN_LEFT = 3,
   DBX_JOIN_RIGHT = 4, DBX_JOIN_RIGHT_SEMI = 5, DBX_JOIN_RIGHT_ANTI = 6, DBX_JOIN_FULL = 7
@@ -232,6 +244,9 @@ typedef struct dbx_join_params {
   int32_t probe_key_col; /* key column index in probe blocks */
   int32_t n_build_cols;  /* dbx_op_create's input_types = build schema (n_build_cols) then probe schema */
   int64_t expected_build_rows; /* hint; 0 = unknown */
+  int32_t n_extra_keys;  /* 0 .. DBX_MAX_JOIN_KEYS - 1 further key pairs */
+  int32_t extra_build_key_cols[DBX_MAX_JOIN_KEYS - 1];
+  int32_t extra_probe_key_cols[DBX_MAX_JOIN_KEYS - 1];
 } dbx_join_params;
 
 /* -------------------------------------------------------- vector distance */

@@ -576,7 +576,9 @@ class AggPartialOp : public Op {
   const char* kernel_variant() override {
     variant_text = jit_status;
     if (partitioned_chunks || partition_fallbacks)
-      variant_text += "; two-pass (partitioned by table region) chunks: " + std::to_string(partitioned_chunks) + ", one-pass fallbacks (skew): " + std::to_string(partition_fallbacks);
+      variant_text += "; two-pass (partitioned by table slice) chunks: " + std::to_string(partitioned_chunks) + " (pass 2 in shared memory: " +
+                      std::to_string(slice_chunks) + ", in L2 regions: " + std::to_string(partitioned_chunks - slice_chunks) +
+                      "), one-pass fallbacks (skew): " + std::to_string(partition_fallbacks);
     return variant_text.c_str();
   }
   // Ask for kernels compiled for this plan (grouped plans without TMA pairs).  Failure is not an
@@ -666,8 +668,10 @@ class AggPartialOp : public Op {
     return DBX_OK;
   }
 
+  int64_t prev_query_groups = 0;  // groups of the query before the last reset (exact at its last counter read)
   int32_t reset() override {
     if (batch_open) { batch_open = false; batch_rows = 0; DBX_TRY(stager.join_aux()); DBX_TRY(stager.end()); }
+    prev_query_groups = groups_known;
     table_ready = false;
     DBX_TRY(ensure_table());
     groups_known = plan.grouped ? 0 : 1;
@@ -981,8 +985,9 @@ class AggPartialOp : public Op {
   // defaults sized to the 50 MB L2: tables beyond ~80% of it go two-pass, in regions of ~40% of it
   int64_t part_threshold = getenv("DBX_AGG_PARTITION_BYTES") ? atoll(getenv("DBX_AGG_PARTITION_BYTES")) : (40LL << 20);
   int64_t part_region_bytes = getenv("DBX_AGG_REGION_BYTES") ? atoll(getenv("DBX_AGG_REGION_BYTES")) : (20LL << 20);
-  int64_t partitioned_chunks = 0, partition_fallbacks = 0;
+  int64_t partitioned_chunks = 0, partition_fallbacks = 0, slice_chunks = 0;
   static constexpr int64_t kPartChunkRows = 1LL << 28;
+  static constexpr int kMaxRegions = 64;  // partitions of the L2-region pass 2
   bool partition_eligible(const DevCol* cols, int64_t m) const {
     if (!plan.grouped || plan.key_words != 1 || plan.n_pairs > 0 || part_threshold <= 0) return false;
     if ((int64_t)table.bytes() <= part_threshold || m < (1 << 16)) return false;
@@ -1019,20 +1024,49 @@ class AggPartialOp : public Op {
     cudaGetLastError();
   }
   template <int NS>
-  void launch_partition(const AggKernelParams& kp, const PartitionOut& po) {
-    static std::atomic<bool> attr_set[64];
-    const size_t smem = (size_t)(NS + 1) * kTileRows * 8;
-    if (device >= 0 && device < 64 && !attr_set[device]) {
+  int32_t launch_partition(const AggKernelParams& kp, const PartitionOut& po) {
+    static std::atomic<int> per_sm[64];  // resident CTAs per SM, 0: not asked yet
+    const size_t smem = partition_smem_bytes<NS>();
+    if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
+    if (!per_sm[device]) {
       cudaFuncSetAttribute(filter_partition_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      int n = 0;
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, filter_partition_kernel<NS>, kBlock, smem);
+      per_sm[device] = std::max(1, n);
+    }
+    // one resident wave: a CTA copies its survivors out only every few tiles, more CTAs would only add partial batches
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * per_sm[device]));
+    filter_partition_kernel<NS><<<grid, kBlock, smem, stream>>>(kp, po);
+    return DBX_OK;
+  }
+  template <int NS>
+  int32_t launch_slice_agg(const AggKernelParams& kp, const SliceIn& si, int n_parts, size_t smem) {
+    static std::atomic<bool> attr_set[64];
+    if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
+    if (!attr_set[device]) {
+      cudaFuncSetAttribute(slice_agg_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSliceBytes);
       attr_set[device] = true;
     }
-    filter_partition_kernel<NS><<<grid_for_rows(kp.n_rows), kBlock, smem, stream>>>(kp, po);
+    slice_agg_kernel<NS><<<n_parts, kSliceBlock, smem, stream>>>(kp, si);
+    return DBX_OK;
+  }
+  // Slots per shared-memory slice of the table (whole buckets, a power of two), or 0 when the table
+  // has more slices than pass 1 can partition into, or when the groups (known so far, or of the previous
+  // query) would fill more than half of it: a slice that fills up defers most of its rows, which then
+  // overflow and replay through the fused kernel.  Pass 2 then runs the fused kernel per L2-sized region.
+  int64_t slice_slots() const {
+    if (2 * std::max(groups_known, prev_query_groups) > table.cap) return 0;
+    int64_t s = 4;
+    while (2 * s * 8 * (1 + table.n_words) <= (int64_t)kSliceBytes && 2 * s <= table.cap) s *= 2;
+    return table.cap / s <= kMaxPartitions ? s : 0;
   }
   // rows [row0, row0 + m) in two passes; *done = false when a partition overflowed (skewed keys): the caller takes the one-pass path
   int32_t partitioned_rows(const DevCol* cols, int64_t row0, int64_t m, bool* done) {
     *done = false;
+    const int64_t slice = slice_slots();
     int n_parts = 2;
-    while (n_parts < kMaxPartitions && (int64_t)table.bytes() / n_parts > part_region_bytes) n_parts <<= 1;
+    if (slice) n_parts = (int)(table.cap / slice);
+    else while (n_parts < kMaxRegions && (int64_t)table.bytes() / n_parts > part_region_bytes) n_parts <<= 1;
     const int64_t nb = table.cap >> 2;
     int lg_nb = 0, lg_p = 0;
     while ((1LL << lg_nb) < nb) ++lg_nb;
@@ -1048,15 +1082,15 @@ class AggPartialOp : public Op {
       po.out[s] = (uint64_t*)part_buf[s].p;
     }
     DBX_CUDA_TRY(err, part_cnt.ensure((kMaxPartitions + 1) * 8));
-    DBX_CUDA_TRY(err, part_host.ensure((kMaxPartitions + 1) * 8));
+    DBX_CUDA_TRY(err, part_host.ensure((kMaxPartitions + 3) * 8));  // [P] overflow flag; [kMaxPartitions + 1, + 2] slice_agg_kernel's counts
     DBX_CUDA_TRY(err, cudaMemsetAsync(part_cnt.p, 0, (kMaxPartitions + 1) * 8, stream));
     po.counts = (unsigned long long*)part_cnt.p; po.cap_p = cap_p; po.nb_mask = (uint64_t)(nb - 1);
     po.region_shift = lg_nb - lg_p; po.n_parts = n_parts;
     switch (plan.n_slots) {
-      case 1: launch_partition<1>(kp, po); break; case 2: launch_partition<2>(kp, po); break;
-      case 3: launch_partition<3>(kp, po); break; case 4: launch_partition<4>(kp, po); break;
-      case 5: launch_partition<5>(kp, po); break; case 6: launch_partition<6>(kp, po); break;
-      case 7: launch_partition<7>(kp, po); break; default: launch_partition<8>(kp, po); break;
+      case 1: DBX_TRY(launch_partition<1>(kp, po)); break; case 2: DBX_TRY(launch_partition<2>(kp, po)); break;
+      case 3: DBX_TRY(launch_partition<3>(kp, po)); break; case 4: DBX_TRY(launch_partition<4>(kp, po)); break;
+      case 5: DBX_TRY(launch_partition<5>(kp, po)); break; case 6: DBX_TRY(launch_partition<6>(kp, po)); break;
+      case 7: DBX_TRY(launch_partition<7>(kp, po)); break; default: DBX_TRY(launch_partition<8>(kp, po)); break;
     }
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
@@ -1065,6 +1099,59 @@ class AggPartialOp : public Op {
     const unsigned long long* hc = (const unsigned long long*)part_host.p;
     if (hc[n_parts]) { ++partition_fallbacks; return DBX_OK; }
     no_filter_ = true;
+    int32_t rc = slice ? slice_pass(kp, po, slice, n_parts) : region_pass(n_parts, cap_p);
+    no_filter_ = false;
+    if (rc == DBX_OK) { *done = true; ++partitioned_chunks; slice_chunks += slice ? 1 : 0; }
+    return rc;
+  }
+  // pass 2 in shared memory: one slice_agg_kernel launch, then the deferred rows through the fused kernel
+  DevBuf deferred[kMaxSlots], n_deferred;
+  int32_t slice_pass(AggKernelParams kp, const PartitionOut& po, int64_t slice, int n_parts) {
+    const unsigned long long* hc = (const unsigned long long*)part_host.p;
+    int64_t survivors = 0;
+    for (int pi = 0; pi < n_parts; ++pi) survivors += (int64_t)hc[pi];
+    for (int s = 0; s < plan.n_slots; ++s) DBX_CUDA_TRY(err, deferred[s].ensure((size_t)std::max<int64_t>(survivors, 1) * 8));
+    DBX_CUDA_TRY(err, n_deferred.ensure(16));
+    DBX_CUDA_TRY(err, cudaMemsetAsync(n_deferred.p, 0, 16, stream));
+    SliceIn si;
+    memset(&si, 0, sizeof(si));
+    for (int s = 0; s < plan.n_slots; ++s) si.in[s] = po.out[s];
+    si.counts = po.counts; si.cap_p = po.cap_p; si.slice_slots = slice;
+    for (int s = 0; s < plan.n_slots; ++s) si.deferred[s] = (uint64_t*)deferred[s].p;
+    si.n_deferred = (unsigned long long*)n_deferred.p;
+    kp.table = table.view(nullptr);
+    const size_t smem = (size_t)slice * 8 * (1 + plan.n_words);
+    switch (plan.n_slots) {
+      case 1: DBX_TRY(launch_slice_agg<1>(kp, si, n_parts, smem)); break; case 2: DBX_TRY(launch_slice_agg<2>(kp, si, n_parts, smem)); break;
+      case 3: DBX_TRY(launch_slice_agg<3>(kp, si, n_parts, smem)); break; case 4: DBX_TRY(launch_slice_agg<4>(kp, si, n_parts, smem)); break;
+      case 5: DBX_TRY(launch_slice_agg<5>(kp, si, n_parts, smem)); break; case 6: DBX_TRY(launch_slice_agg<6>(kp, si, n_parts, smem)); break;
+      case 7: DBX_TRY(launch_slice_agg<7>(kp, si, n_parts, smem)); break; default: DBX_TRY(launch_slice_agg<8>(kp, si, n_parts, smem)); break;
+    }
+    count_launch();
+    DBX_CUDA_TRY(err, cudaGetLastError());
+    DBX_CUDA_TRY(err, cudaMemcpyAsync((char*)part_host.p + (kMaxPartitions + 1) * 8, n_deferred.p, 16, cudaMemcpyDeviceToHost, stream));
+    unsigned long long ng = 0, no = 0;
+    DBX_TRY(read_counters(&ng, &no));
+    const int64_t n_def = (int64_t)((const unsigned long long*)part_host.p)[kMaxPartitions + 1];
+    const int64_t n_full = (int64_t)((const unsigned long long*)part_host.p)[kMaxPartitions + 2];
+    // slices at their fill limit: the table holds fewer slots than the groups need; grow it (the rule of
+    // agg_rows' overflow path) before the deferred rows run, instead of letting them find it full
+    if (n_full > 0) DBX_TRY(grow_to(next_pow2(std::max<int64_t>(table.cap * 4, 2 * (int64_t)ng))));
+    if (n_def > 0) {
+      DevCol pc[kMaxSlots];
+      for (int s = 0; s < plan.n_slots; ++s) {
+        memset(&pc[s], 0, sizeof(DevCol));
+        pc[s].dtype = DBX_U64;  // 64-bit images as the loads would have widened them
+        pc[s].data = deferred[s].p;
+      }
+      return agg_rows(pc, 0, n_def);
+    }
+    if ((int64_t)ng * 2 > table.cap) DBX_TRY(grow_to(next_pow2(4 * (int64_t)ng)));
+    return DBX_OK;
+  }
+  // pass 2 through the fused kernel, one launch per partition, with the partition's table region pinned in L2
+  int32_t region_pass(int n_parts, int64_t cap_p) {
+    const unsigned long long* hc = (const unsigned long long*)part_host.p;
     int32_t rc = DBX_OK;
     const int64_t cap_at_start = table.cap;
     for (int pi = 0; pi < n_parts && rc == DBX_OK; ++pi) {
@@ -1084,9 +1171,7 @@ class AggPartialOp : public Op {
       }
       rc = agg_rows(pc, 0, cnt);
     }
-    no_filter_ = false;
     region_window(nullptr, 0);
-    if (rc == DBX_OK) { *done = true; ++partitioned_chunks; }
     return rc;
   }
 

@@ -424,12 +424,22 @@ __device__ __forceinline__ uint64_t hot_identity(int op) {
   if (op == UPD_MIN_U64 || op == UPD_MIN_F64) return ~0ULL;
   return 0;  // counters, sums (+0.0), unsigned / ordered-float maxima
 }
+// 64-bit add to a shared-memory word as native 32-bit shared atomics (a 64-bit shared atomicAdd is a
+// compare-and-swap loop on sm_90): low half, then the high half plus the low half's carry.  The word is
+// exact (mod 2^64) once every add has completed; nothing reads it in between.
+__device__ __forceinline__ void smem_add_u64(uint64_t* w, uint64_t v) {
+  unsigned int* h = reinterpret_cast<unsigned int*>(w);
+  const unsigned int lo = (unsigned int)v, hi = (unsigned int)(v >> 32);
+  const unsigned int old = atomicAdd(h, lo);
+  const unsigned int up = hi + (old + lo < old ? 1u : 0u);
+  if (up) atomicAdd(h + 1, up);
+}
 __device__ __forceinline__ void hot_update(int op, uint64_t* w, uint64_t val, bool valid) {
-  if (op == UPD_INC) { atomicAdd((unsigned long long*)w, 1ULL); return; }
+  if (op == UPD_INC) { smem_add_u64(w, 1); return; }
   if (!valid) return;
-  if (op == UPD_ADD_INT) { atomicAdd((unsigned long long*)w, (unsigned long long)val); return; }
+  if (op == UPD_ADD_INT) { smem_add_u64(w, val); return; }
   if (op == UPD_ADD_F64) { atomicAdd((double*)w, __longlong_as_double((long long)val)); return; }
-  if (op == UPD_INC_VALID) { atomicAdd((unsigned long long*)w, 1ULL); return; }
+  if (op == UPD_INC_VALID) { smem_add_u64(w, 1); return; }
   if (op == UPD_MIN_S64) { atomicMin((long long*)w, (long long)val); return; }
   if (op == UPD_MAX_S64) { atomicMax((long long*)w, (long long)val); return; }
   if (op == UPD_MIN_U64) { atomicMin((unsigned long long*)w, (unsigned long long)val); return; }
@@ -712,95 +722,327 @@ __global__ void __launch_bounds__(kBlock, 4) filter_group_agg_wide_kernel(const 
 // Tables larger than L2 (>= ~1.5e6 groups of configs[1]'s shape) turn every reduction into a DRAM
 // round trip (2e6 / 1e7 keys: 28 / 44 ms per 1e9 rows instead of 7.6).  For those the operator makes
 // two passes (SURVEY 3.1's fallback): this kernel filters the rows and scatters the survivors'
-// slot values into P partitions by TABLE REGION — region = the top bits of the row's bucket index —
-// and the fused kernel then aggregates one partition at a time, touching only 1/P of the table, which
-// stays in L2.  The table, the final merge and the exchange are unchanged; only the order in which
-// rows reach the table differs.  Per 1024-row tile a CTA counts its rows per region in shared memory,
-// reserves one run per region with one global atomic each, and writes the rows of a region next to
-// each other (runs of ~sel * 1024 / P rows: full sectors for L2 to combine).
-constexpr int kMaxPartitions = 64;
+// slot values into P partitions by TABLE SLICE — slice = the top bits of the row's bucket index —
+// and pass 2 aggregates each partition against its slice of the table only (slice_agg_kernel: the
+// slice in shared memory; tables with too many slices for that: the fused kernel with the slice held
+// in L2).  The table, the final merge and the exchange are unchanged; only the order in which rows
+// reach the table differs.
+//
+// With hundreds of partitions a 1024-row tile has less than one surviving row per partition, so a CTA
+// collects the survivors of several tiles in shared memory (unsorted, each tagged with its partition
+// and its rank inside the partition) before it reserves one run per non-empty partition with one
+// global atomic each and copies the rows out in partition order: consecutive threads store
+// consecutive addresses of a run, and runs of one partition from different CTAs are reserved next to
+// each other, so L2 completes the sectors before they reach DRAM.
+constexpr int kMaxPartitions = 1024;
 struct PartitionOut {
   uint64_t* out[kMaxSlots];       // per slot: [P][cap_p] 64-bit images
   unsigned long long* counts;     // [P] rows written per partition; [P] = overflow flag
   int64_t cap_p;
   uint64_t nb_mask;               // (cap >> 2) - 1
-  int32_t region_shift;           // region = (hash & nb_mask) >> region_shift
+  int32_t region_shift;           // partition = (hash & nb_mask) >> region_shift
   int32_t n_parts;
 };
+// survivors a CTA collects before it copies them out (about 100 KB of shared memory: two CTAs per SM)
 template <int NS>
-__global__ void __launch_bounds__(kBlock, 4) filter_partition_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ PartitionOut po) {
-  // dynamic shared memory: [NS][kTileRows] staged slot values ordered by region, then [kTileRows] destinations
+constexpr int partition_stash_rows() { return NS <= 3 ? 3072 : (NS <= 5 ? 2048 : 1024); }
+template <int NS>
+constexpr size_t partition_smem_bytes() { return (size_t)partition_stash_rows<NS>() * (8 * NS + 4 + 2); }
+
+// GROUP BY key of row j of a thread's tile, for rows without validity (the partitioned path only
+// takes columns without NULLs, so a packed key never carries a NULL flag)
+template <int NS>
+__device__ __forceinline__ uint64_t plain_row_key(const AggKernelParams& p, const RowVals (&vals)[NS], int j) {
+  uint64_t key = 0;
+  if (p.n_key_parts > 1) {
+    for (int k = 0; k < p.n_key_parts; ++k) { const KeyPartDev kp = p.key_parts[k]; key |= (pick<NS>(vals, kp.slot, j) & kp.mask) << kp.shift; }
+  } else {
+    key = pick<NS>(vals, p.key_slot, j);
+    if (p.key_is_float) key = canonical_float_key(key);
+  }
+  return key;
+}
+
+// exclusive prefix sum of cnt[0, n) into off[0, n), n <= 4 * kBlock; ends with the block synchronised
+static_assert(kMaxPartitions <= 4 * kBlock, "block_exclusive_scan: four counts per thread");
+__device__ __forceinline__ void block_exclusive_scan(const unsigned int* cnt, unsigned int* off, int n) {
+  __shared__ unsigned int s_warp[kWarpsPerBlock];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int per = (n + kBlock - 1) / kBlock;
+  unsigned int loc[4], sum = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int i = threadIdx.x * per + q;
+    loc[q] = (q < per && i < n) ? cnt[i] : 0u;
+    sum += loc[q];
+  }
+  unsigned int inc = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int v = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += v;
+  }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  unsigned int ex = inc - sum;
+  for (int w = 0; w < warp; ++w) ex += s_warp[w];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int i = threadIdx.x * per + q;
+    if (q < per && i < n) off[i] = ex;
+    ex += loc[q];
+  }
+  __syncthreads();
+}
+
+template <int NS>
+__global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ PartitionOut po) {
+  constexpr int R = partition_stash_rows<NS>();
+  // dynamic shared memory: [NS][R] survivors in arrival order, [R] tags (partition << 16 | rank), [R] copy-out order
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  uint64_t* stage = reinterpret_cast<uint64_t*>(smem_raw);
-  unsigned long long* dst = reinterpret_cast<unsigned long long*>(smem_raw) + (size_t)NS * kTileRows;
+  uint64_t* stash = reinterpret_cast<uint64_t*>(smem_raw);
+  uint32_t* tag = reinterpret_cast<uint32_t*>(stash + (size_t)NS * R);
+  uint16_t* perm = reinterpret_cast<uint16_t*>(tag + R);
   __shared__ unsigned int s_cnt[kMaxPartitions];
-  __shared__ unsigned int s_off[kMaxPartitions + 1];
+  __shared__ unsigned int s_off[kMaxPartitions];
   __shared__ unsigned long long s_base[kMaxPartitions];
+  __shared__ unsigned int s_wcnt[2][kWarpsPerBlock];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t lt_mask = (1u << lane) - 1;
   const int64_t n_tiles = (p.n_rows + kTileRows - 1) / kTileRows;
   const uint64_t pol = make_policy_evict_first();
+  for (int r = threadIdx.x; r < po.n_parts; r += kBlock) s_cnt[r] = 0;
+  __syncthreads();
+  int n_stash = 0;  // block-uniform
+  int parity = 0;
   RowVals vals[NS];
   uint32_t vmask[NS];
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    if (threadIdx.x < kMaxPartitions) s_cnt[threadIdx.x] = 0;
-    __syncthreads();
+  int64_t tile = blockIdx.x;
+  if (tile < n_tiles) {
+#pragma unroll
+    for (int s = 0; s < NS; ++s) load_slot<false>(p.cols[s], tile * kTileRows, p.n_rows, nullptr, pol, vals[s], vmask[s]);
+  }
+  for (; tile < n_tiles; tile += gridDim.x) {
     const int64_t tile_base = tile * kTileRows;
     const int64_t r0 = tile_base + (int64_t)kRowsPerThread * threadIdx.x;
-#pragma unroll
-    for (int s = 0; s < NS; ++s) load_slot<false>(p.cols[s], tile_base, p.n_rows, nullptr, pol, vals[s], vmask[s]);
     uint32_t in_range = 0;
 #pragma unroll
     for (int j = 0; j < kRowsPerThread; ++j)
       if (r0 + j < p.n_rows) in_range |= 1u << j;
     const uint32_t sel = eval_predicate<NS>(p, vals, vmask, in_range);
-    int region[kRowsPerThread];
-    unsigned int rank[kRowsPerThread];
+    uint32_t tg[kRowsPerThread], bal[kRowsPerThread];
+    int warp_n = 0;
 #pragma unroll
     for (int j = 0; j < kRowsPerThread; ++j) {
-      region[j] = 0; rank[j] = 0;
+      tg[j] = 0;
       if ((sel >> j) & 1) {
-        uint64_t key = 0;
-        if (p.n_key_parts > 1) {
-          for (int k = 0; k < p.n_key_parts; ++k) { const KeyPartDev kp = p.key_parts[k]; key |= (pick<NS>(vals, kp.slot, j) & kp.mask) << kp.shift; }
-        } else {
-          key = pick<NS>(vals, p.key_slot, j);
-          if (p.key_is_float) key = canonical_float_key(key);
+        const uint64_t key = plain_row_key<NS>(p, vals, j);
+        const int part = key == kEmptyKey ? 0 : (int)((agg_hash_u64(key) & po.nb_mask) >> po.region_shift);
+        tg[j] = ((uint32_t)part << 16) | atomicAdd(&s_cnt[part], 1u);
+      }
+      bal[j] = __ballot_sync(0xffffffffu, (sel >> j) & 1);
+      warp_n += __popc(bal[j]);
+    }
+    // stash positions: warps in order, rows of a warp in ballot order (s_wcnt alternates between two
+    // buffers, so a warp that runs ahead into the next tile never overwrites counts still being read)
+    if (lane == 0) s_wcnt[parity][warp] = warp_n;
+    __syncthreads();
+    int pos = n_stash, total = 0;
+    for (int w = 0; w < kWarpsPerBlock; ++w) {
+      const int c = s_wcnt[parity][w];
+      if (w < warp) pos += c;
+      total += c;
+    }
+    parity ^= 1;
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j) {
+      if ((sel >> j) & 1) {
+        const int i = pos + __popc(bal[j] & lt_mask);
+#pragma unroll
+        for (int s = 0; s < NS; ++s) stash[(size_t)s * R + i] = vals[s].v[j];
+        tag[i] = tg[j];
+      }
+      pos += __popc(bal[j]);
+    }
+    n_stash += total;
+    // the next tile's loads fly while this one is stashed and copied out
+    const int64_t next = tile + gridDim.x;
+    if (next < n_tiles) {
+#pragma unroll
+      for (int s = 0; s < NS; ++s) load_slot<false>(p.cols[s], next * kTileRows, p.n_rows, nullptr, pol, vals[s], vmask[s]);
+    }
+    if (n_stash + kTileRows <= R && next < n_tiles) continue;
+    // ---- copy out the collected survivors
+    __syncthreads();
+    block_exclusive_scan(s_cnt, s_off, po.n_parts);
+    for (int r = threadIdx.x; r < po.n_parts; r += kBlock) {
+      const unsigned int c = s_cnt[r];
+      s_base[r] = c ? atomicAdd(&po.counts[r], (unsigned long long)c) : 0ULL;
+    }
+    for (int i = threadIdx.x; i < n_stash; i += kBlock) perm[s_off[tag[i] >> 16] + (tag[i] & 0xFFFF)] = (uint16_t)i;
+    __syncthreads();
+    for (int li = threadIdx.x; li < n_stash; li += kBlock) {
+      const int i = perm[li];
+      const uint32_t part = tag[i] >> 16;
+      const unsigned long long at = s_base[part] + (tag[i] & 0xFFFF);
+      if (at >= (unsigned long long)po.cap_p) { po.counts[po.n_parts] = 1; continue; }  // the host falls back to the one-pass path
+      const unsigned long long d = (unsigned long long)part * (unsigned long long)po.cap_p + at;
+#pragma unroll
+      for (int s = 0; s < NS; ++s) po.out[s][d] = stash[(size_t)s * R + i];
+    }
+    for (int r = threadIdx.x; r < po.n_parts; r += kBlock) s_cnt[r] = 0;
+    n_stash = 0;
+    __syncthreads();  // shared buffers are reused by the next tiles
+  }
+}
+
+// ---------------------------------------------------------------- pass 2: one CTA per table slice
+// CTA i aggregates partition i against slice i of the table (slice_slots consecutive slots = whole
+// buckets) held in shared memory: the slice's keys and state words are loaded from the table, the
+// partition's rows are streamed from pass 1's buffers, every row is probed in the slice in the same
+// linear bucket order as find_or_insert_slow and updates its group with the shared-memory atomics of
+// hot_update, and the slice is stored back with plain stores (no other CTA touches it).  A row is
+// deferred to a list, which the fused kernel then runs against the whole table, when its probe
+// would leave the slice (this includes the wrap from the last bucket to bucket 0), when it reaches
+// probe_limit (or kSliceProbes), or when its key is the EMPTY pattern: these are the only rows this
+// kernel could place somewhere a global probe would not.  As nothing is ever deleted, every key keeps
+// exactly one slot.  A row whose key is new is also deferred once the slice holds kSliceFillNum /
+// kSliceFillDen of its slots: a table with more groups than it was sized for then stops filling here,
+// and the host grows it before the deferred rows run (a full table would make each of them walk
+// probe_limit buckets before it overflows).  Any deferred row is probed globally, so deferring more
+// rows never changes a result.  The deferred rows' values are copied to a compact list, so the fused
+// kernel reads them directly.
+//
+// kSliceBlock threads keep two groups of rows in registers (the next one is in flight): plans with 7
+// or 8 input slots exceed the 128 registers this allows and spill a few words (ptxas: 116 / 404 B).
+constexpr int kSliceBlock = 512;
+constexpr int kSliceFillNum = 3, kSliceFillDen = 4;
+// Buckets a row probes in its slice before it is deferred.  Below the load-factor budget chains this
+// long are rare; a slice that fills up (more groups than the table was sized for) defers its rows after
+// a few probes instead of walking every full bucket to the slice's end.
+constexpr int kSliceProbes = 8;
+constexpr size_t kSliceBytes = 128 << 10;  // shared memory for one slice: keys + state words
+struct SliceIn {
+  const uint64_t* in[kMaxSlots];  // pass 1's partitions: per slot [P][cap_p]
+  const unsigned long long* counts;
+  int64_t cap_p;
+  int64_t slice_slots;
+  uint64_t* deferred[kMaxSlots];  // per slot: the deferred rows' values, in no particular order
+  unsigned long long* n_deferred; // [0] deferred rows, [1] slices that reached the fill limit
+};
+
+template <int NS>
+__device__ __forceinline__ void slice_load_rows(const SliceIn& si, int64_t base, int64_t r0, int64_t n, uint64_t pol, RowVals (&vals)[NS]) {
+  if (r0 + kRowsPerThread <= n) {
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+      const u64x4 q = ld_stream_256(si.in[s] + base + r0);
+      vals[s].v[0] = q.x; vals[s].v[1] = q.y; vals[s].v[2] = q.z; vals[s].v[3] = q.w;
+    }
+  } else {
+#pragma unroll
+    for (int s = 0; s < NS; ++s)
+#pragma unroll
+      for (int j = 0; j < kRowsPerThread; ++j) vals[s].v[j] = r0 + j < n ? ld_stream_u64(si.in[s] + base + r0 + j, pol) : 0;
+  }
+}
+
+template <int NS>
+__global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ SliceIn si) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ unsigned int s_fill, s_fill0;  // occupied slots of the slice: now, and when it was loaded
+  const TableDev& t = p.table;
+  const int nw = t.n_words;
+  const int64_t S = si.slice_slots;
+  uint64_t* skeys = reinterpret_cast<uint64_t*>(smem_raw);
+  uint64_t* sst = skeys + S;  // state word w of slot i at sst[i * nw + w]
+  const int64_t slot0 = (int64_t)blockIdx.x * S;
+  if (threadIdx.x == 0) s_fill = s_fill0 = 0;
+  __syncthreads();
+  unsigned int occupied = 0;
+  for (int64_t i = threadIdx.x; i < S; i += kSliceBlock) {
+    skeys[i] = t.keys[slot0 + i];
+    occupied += skeys[i] != kEmptyKey;
+  }
+  if (occupied) { atomicAdd(&s_fill, occupied); atomicAdd(&s_fill0, occupied); }
+  for (int64_t e = threadIdx.x; e < S * nw; e += kSliceBlock) {
+    const int64_t i = e / nw;
+    sst[e] = *word_ptr(t, slot0 + i, (int)(e - i * nw));
+  }
+  __syncthreads();
+  const unsigned int fill_limit = (unsigned int)(S * kSliceFillNum / kSliceFillDen);
+  volatile unsigned int* vfill = &s_fill;
+
+  const int64_t n = (int64_t)si.counts[blockIdx.x];
+  const int64_t base = (int64_t)blockIdx.x * si.cap_p;
+  const int64_t nbs = S >> 2;  // buckets per slice
+  const uint64_t nb_mask = (uint64_t)(t.cap >> 2) - 1;
+  const uint64_t pol = make_policy_evict_first();
+  volatile uint64_t* vkeys = skeys;
+  bool hit_limit = false;
+  constexpr int64_t kStep = (int64_t)kRowsPerThread * kSliceBlock;
+  const int lane = threadIdx.x & 31;
+  RowVals vals[NS], next[NS];
+  // the loop runs warp-uniformly (lanes past the end idle), so deferred rows are reserved once per warp
+  const int64_t warp_r0 = (int64_t)kRowsPerThread * (threadIdx.x & ~31);
+  int64_t r0 = (int64_t)kRowsPerThread * threadIdx.x;
+  if (r0 < n) slice_load_rows<NS>(si, base, r0, n, pol, vals);
+  for (int64_t w0 = warp_r0; w0 < n; w0 += kStep, r0 += kStep) {
+    if (r0 + kStep < n) slice_load_rows<NS>(si, base, r0 + kStep, n, pol, next);  // in flight while this group is aggregated
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j) {
+      const bool live = r0 + j < n;
+      const uint64_t key = live ? plain_row_key<NS>(p, vals, j) : 0;
+      int64_t slot = -1;
+      if (live && key != kEmptyKey) {
+        int64_t lb = (int64_t)(agg_hash_u64(key) & nb_mask) - (int64_t)blockIdx.x * nbs;
+        int probes = 0;
+        while (probes < min(t.probe_limit, kSliceProbes)) {
+          const uint64_t k0 = vkeys[4 * lb], k1 = vkeys[4 * lb + 1], k2 = vkeys[4 * lb + 2], k3 = vkeys[4 * lb + 3];
+          const int m = k0 == key ? 0 : (k1 == key ? 1 : (k2 == key ? 2 : (k3 == key ? 3 : -1)));
+          if (m >= 0) { slot = 4 * lb + m; break; }
+          const int e = k0 == kEmptyKey ? 0 : (k1 == kEmptyKey ? 1 : (k2 == kEmptyKey ? 2 : (k3 == kEmptyKey ? 3 : -1)));
+          if (e >= 0) {
+            if (*vfill >= fill_limit) { hit_limit = true; break; }  // a new group for a full slice: deferred
+            const unsigned long long old = atomicCAS((unsigned long long*)(skeys + 4 * lb + e), (unsigned long long)kEmptyKey, (unsigned long long)key);
+            if (old == kEmptyKey) { atomicAdd(&s_fill, 1u); slot = 4 * lb + e; break; }
+            if (old == key) { slot = 4 * lb + e; break; }
+            continue;  // another key took the slot: look at this bucket again (it has one EMPTY slot less)
+          }
+          if (++lb == nbs) break;  // the probe leaves the slice
+          ++probes;
         }
-        region[j] = key == kEmptyKey ? 0 : (int)((agg_hash_u64(key) & po.nb_mask) >> po.region_shift);
-        rank[j] = atomicAdd(&s_cnt[region[j]], 1u);
+      }
+      const bool defer = live && slot < 0;
+      const unsigned dm = __ballot_sync(0xffffffffu, defer);
+      if (dm) {
+        unsigned long long d = 0;
+        if (lane == 0) d = atomicAdd(si.n_deferred, (unsigned long long)__popc(dm));
+        d = __shfl_sync(0xffffffffu, d, 0) + __popc(dm & ((1u << lane) - 1));
+        if (defer) {
+#pragma unroll
+          for (int s = 0; s < NS; ++s) si.deferred[s][d] = vals[s].v[j];
+        }
+      }
+      if (slot < 0) continue;
+      uint64_t* w = sst + slot * nw;
+      for (int u = 0; u < p.n_updates; ++u) {
+        const UpdateDev ud = p.upd[u];
+        hot_update(ud.op, w + ud.word, pick<NS>(vals, ud.slot, j), true);
       }
     }
-    __syncthreads();
-    if (threadIdx.x < po.n_parts) {
-      const unsigned int c = s_cnt[threadIdx.x];
-      s_base[threadIdx.x] = c ? atomicAdd(&po.counts[threadIdx.x], (unsigned long long)c) : 0ULL;
-    }
-    if (threadIdx.x == 0) {
-      unsigned int acc = 0;
-      for (int r = 0; r < po.n_parts; ++r) { s_off[r] = acc; acc += s_cnt[r]; }
-      s_off[po.n_parts] = acc;
-    }
-    __syncthreads();
-    // stage the surviving rows in region order, with the global position of each
 #pragma unroll
-    for (int j = 0; j < kRowsPerThread; ++j) {
-      if (!((sel >> j) & 1)) continue;
-      const unsigned int li = s_off[region[j]] + rank[j];
-      const unsigned long long pos = s_base[region[j]] + rank[j];
-      if (pos >= (unsigned long long)po.cap_p) { po.counts[po.n_parts] = 1; dst[li] = ~0ULL; }  // the host falls back to the one-pass path
-      else dst[li] = (unsigned long long)region[j] * (unsigned long long)po.cap_p + pos;
-#pragma unroll
-      for (int s = 0; s < NS; ++s) stage[(size_t)s * kTileRows + li] = vals[s].v[j];
-    }
-    __syncthreads();
-    // copy out: consecutive staged rows of a region go to consecutive addresses (whole sectors per warp)
-    const unsigned int n_sel = s_off[po.n_parts];
-    for (unsigned int li = threadIdx.x; li < n_sel; li += kBlock) {
-      const unsigned long long d = dst[li];
-      if (d == ~0ULL) continue;
-#pragma unroll
-      for (int s = 0; s < NS; ++s) po.out[s][d] = stage[(size_t)s * kTileRows + li];
-    }
-    __syncthreads();  // shared buffers are reused by the next tile
+    for (int s = 0; s < NS; ++s) vals[s] = next[s];
+  }
+  const int any_hit = __syncthreads_or(hit_limit);
+  for (int64_t i = threadIdx.x; i < S; i += kSliceBlock) t.keys[slot0 + i] = skeys[i];
+  for (int64_t e = threadIdx.x; e < S * nw; e += kSliceBlock) {
+    const int64_t i = e / nw;
+    *word_ptr(t, slot0 + i, (int)(e - i * nw)) = sst[e];
+  }
+  if (threadIdx.x == 0) {
+    if (s_fill > s_fill0) atomicAdd(t.n_groups, (unsigned long long)(s_fill - s_fill0));
+    if (any_hit) atomicAdd(si.n_deferred + 1, 1ULL);
   }
 }
 

@@ -529,6 +529,22 @@ static size_t kMaxSlotsStageBytes(int ns) {
   }
 }
 
+// dynamic shared memory of the partitioned passes for a run-time slot count: pass 1's stash, pass 2's row buffers
+static size_t partition_smem_for(int ns) {
+  switch (ns) {
+    case 1: return partition_smem_bytes<1>(); case 2: return partition_smem_bytes<2>(); case 3: return partition_smem_bytes<3>();
+    case 4: return partition_smem_bytes<4>(); case 5: return partition_smem_bytes<5>(); case 6: return partition_smem_bytes<6>();
+    case 7: return partition_smem_bytes<7>(); default: return partition_smem_bytes<8>();
+  }
+}
+static size_t slice_stage_bytes_for(int ns) {
+  switch (ns) {
+    case 1: return slice_stage_bytes<1>(); case 2: return slice_stage_bytes<2>(); case 3: return slice_stage_bytes<3>();
+    case 4: return slice_stage_bytes<4>(); case 5: return slice_stage_bytes<5>(); case 6: return slice_stage_bytes<6>();
+    case 7: return slice_stage_bytes<7>(); default: return slice_stage_bytes<8>();
+  }
+}
+
 // ================================================================ partial
 class AggPartialOp : public Op {
  public:
@@ -578,7 +594,9 @@ class AggPartialOp : public Op {
     if (partitioned_chunks || partition_fallbacks)
       variant_text += "; two-pass (partitioned by table slice) chunks: " + std::to_string(partitioned_chunks) + " (pass 2 in shared memory: " +
                       std::to_string(slice_chunks) + ", in L2 regions: " + std::to_string(partitioned_chunks - slice_chunks) +
-                      "), one-pass fallbacks (skew): " + std::to_string(partition_fallbacks);
+                      "), one-pass fallbacks (skew): " + std::to_string(partition_fallbacks) + "; specialised launches: pass 1 " +
+                      std::to_string(part_jit_launches) + " of " + std::to_string(partitioned_chunks + partition_fallbacks) + ", pass 2 " +
+                      std::to_string(slice_jit_launches) + " of " + std::to_string(slice_chunks);
     return variant_text.c_str();
   }
   // Ask for kernels compiled for this plan (grouped plans without TMA pairs).  Failure is not an
@@ -611,6 +629,17 @@ class AggPartialOp : public Op {
       return;
     }
     jit_status = "specialised";
+    // the two passes of the partitioned path: both use more than 48 KB of dynamic shared memory
+    ce = cudaKernelSetAttributeForDevice(jit.part, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)partition_smem_for(plan.n_slots), device);
+    if (ce == cudaSuccess)
+      ce = cudaKernelSetAttributeForDevice(jit.slice, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSliceBytes + slice_stage_bytes_for(plan.n_slots)), device);
+    if (ce != cudaSuccess) drop_two_pass_jit("shared-memory opt-in", ce);
+  }
+  // the partitioned passes go back to the precompiled kernels; the fused kernels stay specialised
+  void drop_two_pass_jit(const char* what, cudaError_t ce) {
+    cudaGetLastError();
+    jit.part = jit.slice = nullptr;
+    jit_status += std::string(" (two-pass: precompiled kernels, ") + what + " of the specialised kernel failed: " + cudaGetErrorString(ce) + ")";
   }
 
   // Pin the hash table in L2 while the column stream passes through: a persisting access-policy
@@ -1023,11 +1052,26 @@ class AggPartialOp : public Op {
     if (!region_window_on) cudaCtxResetPersistingL2Cache();
     cudaGetLastError();
   }
+  int jit_part_per_sm = 0;  // resident CTAs per SM of the specialised pass 1, 0: not asked yet
+  int64_t part_jit_launches = 0, slice_jit_launches = 0;
   template <int NS>
   int32_t launch_partition(const AggKernelParams& kp, const PartitionOut& po) {
     static std::atomic<int> per_sm[64];  // resident CTAs per SM, 0: not asked yet
     const size_t smem = partition_smem_bytes<NS>();
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
+    if (jit.two_pass_ok() && !jit_part_per_sm) {  // the occupancy of the kernel that will run
+      int n = 0;
+      const cudaError_t ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, (const void*)jit.part, kBlock, smem);
+      if (ce == cudaSuccess) jit_part_per_sm = std::max(1, n);
+      else drop_two_pass_jit("occupancy query", ce);
+    }
+    if (jit.two_pass_ok()) {
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * jit_part_per_sm));
+      void* args[] = {(void*)&kp, (void*)&po};
+      const cudaError_t ce = cudaLaunchKernel((const void*)jit.part, dim3(grid), dim3(kBlock), args, smem, stream);
+      if (ce == cudaSuccess) { ++part_jit_launches; return DBX_OK; }
+      drop_two_pass_jit("launch", ce);
+    }
     if (!per_sm[device]) {
       cudaFuncSetAttribute(filter_partition_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       int n = 0;
@@ -1040,11 +1084,18 @@ class AggPartialOp : public Op {
     return DBX_OK;
   }
   template <int NS>
-  int32_t launch_slice_agg(const AggKernelParams& kp, const SliceIn& si, int n_parts, size_t smem) {
+  int32_t launch_slice_agg(const AggKernelParams& kp, const SliceIn& si, int n_parts, size_t slice_bytes) {
     static std::atomic<bool> attr_set[64];
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
+    const size_t smem = slice_bytes + slice_stage_bytes<NS>();  // the slice, then the two row buffers
+    if (jit.two_pass_ok()) {
+      void* args[] = {(void*)&kp, (void*)&si};
+      const cudaError_t ce = cudaLaunchKernel((const void*)jit.slice, dim3(n_parts), dim3(kSliceBlock), args, smem, stream);
+      if (ce == cudaSuccess) { ++slice_jit_launches; return DBX_OK; }
+      drop_two_pass_jit("launch", ce);
+    }
     if (!attr_set[device]) {
-      cudaFuncSetAttribute(slice_agg_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSliceBytes);
+      cudaFuncSetAttribute(slice_agg_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSliceBytes + slice_stage_bytes<NS>()));
       attr_set[device] = true;
     }
     slice_agg_kernel<NS><<<n_parts, kSliceBlock, smem, stream>>>(kp, si);

@@ -1,4 +1,5 @@
-// agg_jit.h — run-time specialisation of the fused filter -> hash-aggregate kernel.
+// agg_jit.h — run-time specialisation of the fused filter -> hash-aggregate kernel and of the two
+// passes of the partitioned aggregation.
 //
 // The reference interprets its plan per block (FilterExecutor + AggregateHashTable dispatch over
 // dynamic `dyn AggregateFunction`s, aggregate_function.rs); the precompiled kernels here interpret
@@ -17,7 +18,10 @@ namespace dbx {
 struct AggJitKernels {
   cudaKernel_t fast = nullptr;  // whole tiles of plain 8-byte columns (FAST)
   cudaKernel_t gen = nullptr;   // any column layout, direct row order
+  cudaKernel_t part = nullptr;  // pass 1 of the partitioned aggregation (filter_partition_body)
+  cudaKernel_t slice = nullptr; // pass 2 in shared memory (slice_agg_body)
   bool ok() const { return fast && gen; }
+  bool two_pass_ok() const { return part && slice; }
 };
 
 // Text of the StaticPlan initialiser for a plan; empty when the plan cannot be specialised.

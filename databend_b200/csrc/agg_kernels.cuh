@@ -717,7 +717,6 @@ __global__ void __launch_bounds__(kBlock, 4) filter_group_agg_wide_kernel(const 
 }
 #endif
 
-#ifndef DBX_JIT  // everything below is compiled offline only
 // ---------------------------------------------------------------- pass 1 of the partitioned aggregation
 // Tables larger than L2 (>= ~1.5e6 groups of configs[1]'s shape) turn every reduction into a DRAM
 // round trip (2e6 / 1e7 keys: 28 / 44 ms per 1e9 rows instead of 7.6).  For those the operator makes
@@ -745,20 +744,21 @@ struct PartitionOut {
 };
 // survivors a CTA collects before it copies them out (about 100 KB of shared memory: two CTAs per SM)
 template <int NS>
-constexpr int partition_stash_rows() { return NS <= 3 ? 3072 : (NS <= 5 ? 2048 : 1024); }
+__host__ __device__ constexpr int partition_stash_rows() { return NS <= 3 ? 3072 : (NS <= 5 ? 2048 : 1024); }
 template <int NS>
-constexpr size_t partition_smem_bytes() { return (size_t)partition_stash_rows<NS>() * (8 * NS + 4 + 2); }
+__host__ __device__ constexpr size_t partition_smem_bytes() { return (size_t)partition_stash_rows<NS>() * (8 * NS + 4 + 2); }
 
 // GROUP BY key of row j of a thread's tile, for rows without validity (the partitioned path only
 // takes columns without NULLs, so a packed key never carries a NULL flag)
 template <int NS>
 __device__ __forceinline__ uint64_t plain_row_key(const AggKernelParams& p, const RowVals (&vals)[NS], int j) {
   uint64_t key = 0;
-  if (p.n_key_parts > 1) {
-    for (int k = 0; k < p.n_key_parts; ++k) { const KeyPartDev kp = p.key_parts[k]; key |= (pick<NS>(vals, kp.slot, j) & kp.mask) << kp.shift; }
+  if (PLN(n_key_parts) > 1) {
+    PLN_UNROLL
+    for (int k = 0; k < PLN(n_key_parts); ++k) { const KeyPartDev kp = PLN(key_parts[k]); key |= (pick<NS>(vals, kp.slot, j) & kp.mask) << kp.shift; }
   } else {
-    key = pick<NS>(vals, p.key_slot, j);
-    if (p.key_is_float) key = canonical_float_key(key);
+    key = pick<NS>(vals, PLN(key_slot), j);
+    if (PLN(key_is_float)) key = canonical_float_key(key);
   }
   return key;
 }
@@ -796,7 +796,7 @@ __device__ __forceinline__ void block_exclusive_scan(const unsigned int* cnt, un
 }
 
 template <int NS>
-__global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ PartitionOut po) {
+__device__ __forceinline__ void filter_partition_body(const AggKernelParams& p, const PartitionOut& po) {
   constexpr int R = partition_stash_rows<NS>();
   // dynamic shared memory: [NS][R] survivors in arrival order, [R] tags (partition << 16 | rank), [R] copy-out order
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -900,8 +900,8 @@ __global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __gri
 // CTA i aggregates partition i against slice i of the table (slice_slots consecutive slots = whole
 // buckets) held in shared memory: the slice's keys and state words are loaded from the table, the
 // partition's rows are streamed from pass 1's buffers, every row is probed in the slice in the same
-// linear bucket order as find_or_insert_slow and updates its group with the shared-memory atomics of
-// hot_update, and the slice is stored back with plain stores (no other CTA touches it).  A row is
+// linear bucket order as find_or_insert_slow and updates its group with shared-memory atomics
+// (slice_update), and the slice is stored back with plain stores (no other CTA touches it).  A row is
 // deferred to a list, which the fused kernel then runs against the whole table, when its probe
 // would leave the slice (this includes the wrap from the last bucket to bucket 0), when it reaches
 // probe_limit (or kSliceProbes), or when its key is the EMPTY pattern: these are the only rows this
@@ -913,15 +913,32 @@ __global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __gri
 // rows never changes a result.  The deferred rows' values are copied to a compact list, so the fused
 // kernel reads them directly.
 //
-// kSliceBlock threads keep two groups of rows in registers (the next one is in flight): plans with 7
-// or 8 input slots exceed the 128 registers this allows and spill a few words (ptxas: 116 / 404 B).
-constexpr int kSliceBlock = 512;
+// The cost of a row is a chain of shared-memory accesses (bucket loads, then atomics whose returned
+// values feed the next step), so what matters is how many rows are in flight per SM.  The partition's
+// rows are therefore copied into shared memory with cp.async in stages of slice_stage_rows<NS>() rows,
+// double-buffered (the next stage is in flight while this one is aggregated), and no row values are
+// held in registers across a stage: kSliceBlock = 1024 threads (32 warps per SM, at most 64 registers)
+// work on a stage.  Each thread takes RPT rows of it and handles them in phases: it loads the first
+// bucket of every row (two 128-bit shared loads each) before it resolves any slot, then issues the
+// updates of all of them update by update, so the atomics of different rows are in flight together.
+constexpr int kSliceBlock = 1024;
 constexpr int kSliceFillNum = 3, kSliceFillDen = 4;
 // Buckets a row probes in its slice before it is deferred.  Below the load-factor budget chains this
 // long are rare; a slice that fills up (more groups than the table was sized for) defers its rows after
 // a few probes instead of walking every full bucket to the slice's end.
 constexpr int kSliceProbes = 8;
-constexpr size_t kSliceBytes = 128 << 10;  // shared memory for one slice: keys + state words
+constexpr size_t kSliceBytes = 128 << 10;       // shared memory for one slice: keys + state words
+constexpr size_t kSliceStageBytes = 96 << 10;   // both row buffers: a full slice and its rows take 224 of the 227 KB a CTA may use
+// rows per stage: a power of two from kSliceBlock / 2 to 2 * kSliceBlock (more rows per thread spill at 64
+// registers), two buffers of NS slots within kSliceStageBytes
+template <int NS>
+__host__ __device__ constexpr int slice_stage_rows() {
+  int r = 2 * kSliceBlock;
+  while (r > kSliceBlock / 2 && (size_t)2 * NS * 8 * r > kSliceStageBytes) r >>= 1;
+  return r;
+}
+template <int NS>
+__host__ __device__ constexpr size_t slice_stage_bytes() { return (size_t)2 * NS * 8 * slice_stage_rows<NS>(); }
 struct SliceIn {
   const uint64_t* in[kMaxSlots];  // pass 1's partitions: per slot [P][cap_p]
   const unsigned long long* counts;
@@ -931,89 +948,194 @@ struct SliceIn {
   unsigned long long* n_deferred; // [0] deferred rows, [1] slices that reached the fill limit
 };
 
-template <int NS>
-__device__ __forceinline__ void slice_load_rows(const SliceIn& si, int64_t base, int64_t r0, int64_t n, uint64_t pol, RowVals (&vals)[NS]) {
-  if (r0 + kRowsPerThread <= n) {
+__device__ __forceinline__ void cp_async_16(void* smem, const void* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
+}
+// Rows [r0, r0 + min(B, n - r0)) of the partition at `base`, every slot, into buf[NS][B] as one cp.async
+// group.  The copy moves whole 16-byte pairs of rows: a partition's buffer holds cap_p >= n rows and cap_p
+// is a multiple of 4, so the pair that holds the last row stays inside it (its other row is not used).
+template <int NS, int B>
+__device__ __forceinline__ void slice_stage_copy(const SliceIn& si, int64_t base, int64_t r0, int64_t n, uint64_t* buf) {
+  const int pairs = (int)((min((int64_t)B, n - r0) + 1) >> 1);
 #pragma unroll
-    for (int s = 0; s < NS; ++s) {
-      const u64x4 q = ld_stream_256(si.in[s] + base + r0);
-      vals[s].v[0] = q.x; vals[s].v[1] = q.y; vals[s].v[2] = q.z; vals[s].v[3] = q.w;
-    }
+  for (int s = 0; s < NS; ++s)
+    for (int c = threadIdx.x; c < pairs; c += kSliceBlock) cp_async_16(buf + (size_t)s * B + 2 * c, si.in[s] + base + r0 + 2 * c);
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// One 32-byte bucket of the slice as two 128-bit shared loads; volatile: other threads insert keys meanwhile.
+__device__ __forceinline__ u64x4 lds_bucket(const uint64_t* b) {
+  u64x4 r;
+  const uint32_t a = (uint32_t)__cvta_generic_to_shared(b);
+  asm volatile("ld.volatile.shared.v2.u64 {%0, %1}, [%2];" : "=l"(r.x), "=l"(r.y) : "r"(a) : "memory");
+  asm volatile("ld.volatile.shared.v2.u64 {%0, %1}, [%2+16];" : "=l"(r.z), "=l"(r.w) : "r"(a) : "memory");
+  return r;
+}
+
+// GROUP BY key of row i of a stage (slot s of row i at st[s * B + i]); no validity, as in plain_row_key
+template <int B>
+__device__ __forceinline__ uint64_t stage_row_key(const AggKernelParams& p, const uint64_t* st, int i) {
+  uint64_t key = 0;
+  if (PLN(n_key_parts) > 1) {
+    PLN_UNROLL
+    for (int k = 0; k < PLN(n_key_parts); ++k) { const KeyPartDev kp = PLN(key_parts[k]); key |= (st[(size_t)kp.slot * B + i] & kp.mask) << kp.shift; }
   } else {
-#pragma unroll
-    for (int s = 0; s < NS; ++s)
-#pragma unroll
-      for (int j = 0; j < kRowsPerThread; ++j) vals[s].v[j] = r0 + j < n ? ld_stream_u64(si.in[s] + base + r0 + j, pol) : 0;
+    key = st[(size_t)PLN(key_slot) * B + i];
+    if (PLN(key_is_float)) key = canonical_float_key(key);
+  }
+  return key;
+}
+
+// The probe of one row from its first bucket lb (contents kb) on: the slot, -1 when the row is deferred
+// because its probe leaves the slice or reaches max_probes, -2 when it is a new group for a slice at
+// its fill limit.
+__device__ __noinline__ int64_t slice_probe(uint64_t* skeys, uint64_t key, int64_t lb, u64x4 kb, int64_t nbs, int max_probes,
+                                            unsigned int* s_fill, unsigned int fill_limit) {
+  int probes = 0;
+  while (true) {
+    const int m = bucket_match(kb, key);
+    if (m >= 0) return 4 * lb + m;
+    const int e = kb.x == kEmptyKey ? 0 : (kb.y == kEmptyKey ? 1 : (kb.z == kEmptyKey ? 2 : (kb.w == kEmptyKey ? 3 : -1)));
+    if (e >= 0) {
+      if (*(volatile unsigned int*)s_fill >= fill_limit) return -2;
+      const unsigned long long old = atomicCAS((unsigned long long*)(skeys + 4 * lb + e), (unsigned long long)kEmptyKey, (unsigned long long)key);
+      if (old == kEmptyKey) { atomicAdd(s_fill, 1u); return 4 * lb + e; }
+      if (old == key) return 4 * lb + e;
+      kb = lds_bucket(skeys + 4 * lb);  // another key took the slot: look at this bucket again (it has one EMPTY slot less)
+      continue;
+    }
+    if (++lb == nbs) return -1;  // the probe leaves the slice
+    if (++probes >= max_probes) return -1;
+    kb = lds_bucket(skeys + 4 * lb);
   }
 }
 
+// One state word of each of a thread's RPT rows (w[r]: the word; bit r of `on`: row r has a slot here).
+// Integer adds are two native 32-bit shared adds plus a carry, as in smem_add_u64, with the low halves of
+// all rows issued before any carry is looked at; the compare-and-swap loops of f64 sums run side by side;
+// minima and maxima use hot_update's shared-memory atomics.
+template <int RPT>
+__device__ __forceinline__ void slice_update(int op, uint64_t* const (&w)[RPT], const uint64_t (&v)[RPT], uint32_t on) {
+  if (op == UPD_INC || op == UPD_INC_VALID || op == UPD_ADD_INT) {
+    unsigned int old[RPT];
+#pragma unroll
+    for (int r = 0; r < RPT; ++r)
+      if ((on >> r) & 1) old[r] = atomicAdd(reinterpret_cast<unsigned int*>(w[r]), op == UPD_ADD_INT ? (unsigned int)v[r] : 1u);
+#pragma unroll
+    for (int r = 0; r < RPT; ++r) {
+      if (!((on >> r) & 1)) continue;
+      const unsigned int lo = op == UPD_ADD_INT ? (unsigned int)v[r] : 1u, hi = op == UPD_ADD_INT ? (unsigned int)(v[r] >> 32) : 0u;
+      const unsigned int up = hi + (old[r] + lo < old[r] ? 1u : 0u);
+      if (up) atomicAdd(reinterpret_cast<unsigned int*>(w[r]) + 1, up);
+    }
+    return;
+  }
+  if (op == UPD_ADD_F64) {
+    unsigned long long cur[RPT];
+#pragma unroll
+    for (int r = 0; r < RPT; ++r)
+      if ((on >> r) & 1) cur[r] = *reinterpret_cast<volatile unsigned long long*>(w[r]);
+    for (uint32_t pend = on; pend;) {
+#pragma unroll
+      for (int r = 0; r < RPT; ++r) {
+        if (!((pend >> r) & 1)) continue;
+        const unsigned long long nv = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur[r]) + __longlong_as_double((long long)v[r]));
+        const unsigned long long o = atomicCAS(reinterpret_cast<unsigned long long*>(w[r]), cur[r], nv);
+        if (o == cur[r]) pend &= ~(1u << r);
+        cur[r] = o;
+      }
+    }
+    return;
+  }
+#pragma unroll
+  for (int r = 0; r < RPT; ++r)
+    if ((on >> r) & 1) hot_update(op, w[r], v[r], true);
+}
+
 template <int NS>
-__global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ SliceIn si) {
+__device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const SliceIn& si) {
+  constexpr int B = slice_stage_rows<NS>();
+  constexpr int RPT = B >= kSliceBlock ? B / kSliceBlock : 1;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ unsigned int s_fill, s_fill0;  // occupied slots of the slice: now, and when it was loaded
   const TableDev& t = p.table;
-  const int nw = t.n_words;
+  // the two-pass path has no paired words: the nw state words of a slot are one row-major entry, and the
+  // slice's entries are one contiguous run of the table
+  const int nw = PLN_TABLE(n_single);
   const int64_t S = si.slice_slots;
   uint64_t* skeys = reinterpret_cast<uint64_t*>(smem_raw);
-  uint64_t* sst = skeys + S;  // state word w of slot i at sst[i * nw + w]
+  uint64_t* sst = skeys + S;                 // state word w of slot i at sst[i * nw + w]
+  uint64_t* stage = sst + S * nw;            // two buffers of [NS][B] row values
   const int64_t slot0 = (int64_t)blockIdx.x * S;
-  if (threadIdx.x == 0) s_fill = s_fill0 = 0;
-  __syncthreads();
-  unsigned int occupied = 0;
-  for (int64_t i = threadIdx.x; i < S; i += kSliceBlock) {
-    skeys[i] = t.keys[slot0 + i];
-    occupied += skeys[i] != kEmptyKey;
-  }
-  if (occupied) { atomicAdd(&s_fill, occupied); atomicAdd(&s_fill0, occupied); }
-  for (int64_t e = threadIdx.x; e < S * nw; e += kSliceBlock) {
-    const int64_t i = e / nw;
-    sst[e] = *word_ptr(t, slot0 + i, (int)(e - i * nw));
-  }
-  __syncthreads();
-  const unsigned int fill_limit = (unsigned int)(S * kSliceFillNum / kSliceFillDen);
-  volatile unsigned int* vfill = &s_fill;
-
   const int64_t n = (int64_t)si.counts[blockIdx.x];
   const int64_t base = (int64_t)blockIdx.x * si.cap_p;
+  const int64_t n_stages = (n + B - 1) / B;
+  if (n_stages > 0) slice_stage_copy<NS, B>(si, base, 0, n, stage);  // in flight while the slice is loaded
+  if (threadIdx.x == 0) s_fill = s_fill0 = 0;
+  __syncthreads();
+  ulonglong2* gkeys = reinterpret_cast<ulonglong2*>(t.keys + slot0);
+  ulonglong2* gst = reinterpret_cast<ulonglong2*>(t.states + t.row_base + slot0 * nw);
+  unsigned int occupied = 0;
+#pragma unroll 2
+  for (int64_t i = threadIdx.x; i < S / 2; i += kSliceBlock) {
+    const ulonglong2 k = gkeys[i];
+    reinterpret_cast<ulonglong2*>(skeys)[i] = k;
+    occupied += (k.x != kEmptyKey ? 1u : 0u) + (k.y != kEmptyKey ? 1u : 0u);
+  }
+  if (occupied) { atomicAdd(&s_fill, occupied); atomicAdd(&s_fill0, occupied); }
+#pragma unroll 4
+  for (int64_t e = threadIdx.x; e < S * nw / 2; e += kSliceBlock) reinterpret_cast<ulonglong2*>(sst)[e] = gst[e];
+  const unsigned int fill_limit = (unsigned int)(S * kSliceFillNum / kSliceFillDen);
   const int64_t nbs = S >> 2;  // buckets per slice
   const uint64_t nb_mask = (uint64_t)(t.cap >> 2) - 1;
-  const uint64_t pol = make_policy_evict_first();
-  volatile uint64_t* vkeys = skeys;
-  bool hit_limit = false;
-  constexpr int64_t kStep = (int64_t)kRowsPerThread * kSliceBlock;
+  const int max_probes = min(t.probe_limit, kSliceProbes);
   const int lane = threadIdx.x & 31;
-  RowVals vals[NS], next[NS];
-  // the loop runs warp-uniformly (lanes past the end idle), so deferred rows are reserved once per warp
-  const int64_t warp_r0 = (int64_t)kRowsPerThread * (threadIdx.x & ~31);
-  int64_t r0 = (int64_t)kRowsPerThread * threadIdx.x;
-  if (r0 < n) slice_load_rows<NS>(si, base, r0, n, pol, vals);
-  for (int64_t w0 = warp_r0; w0 < n; w0 += kStep, r0 += kStep) {
-    if (r0 + kStep < n) slice_load_rows<NS>(si, base, r0 + kStep, n, pol, next);  // in flight while this group is aggregated
+  bool hit_limit = false;
+  for (int64_t k = 0; k < n_stages; ++k) {
+    const uint64_t* st = stage + (size_t)(k & 1) * NS * B;
+    if (k + 1 < n_stages) {
+      slice_stage_copy<NS, B>(si, base, (k + 1) * B, n, stage + (size_t)((k + 1) & 1) * NS * B);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncthreads();  // this stage's rows (and, the first time, the slice) are visible to every thread
+    const int m = (int)min((int64_t)B, n - k * B);
+    // phase 1: the first bucket of every row, then the slots
+    uint64_t key[RPT];
+    int64_t lb[RPT];
+    u64x4 kb[RPT];
+    uint32_t probe = 0;  // rows with a key to probe (the EMPTY pattern is deferred)
 #pragma unroll
-    for (int j = 0; j < kRowsPerThread; ++j) {
-      const bool live = r0 + j < n;
-      const uint64_t key = live ? plain_row_key<NS>(p, vals, j) : 0;
-      int64_t slot = -1;
-      if (live && key != kEmptyKey) {
-        int64_t lb = (int64_t)(agg_hash_u64(key) & nb_mask) - (int64_t)blockIdx.x * nbs;
-        int probes = 0;
-        while (probes < min(t.probe_limit, kSliceProbes)) {
-          const uint64_t k0 = vkeys[4 * lb], k1 = vkeys[4 * lb + 1], k2 = vkeys[4 * lb + 2], k3 = vkeys[4 * lb + 3];
-          const int m = k0 == key ? 0 : (k1 == key ? 1 : (k2 == key ? 2 : (k3 == key ? 3 : -1)));
-          if (m >= 0) { slot = 4 * lb + m; break; }
-          const int e = k0 == kEmptyKey ? 0 : (k1 == kEmptyKey ? 1 : (k2 == kEmptyKey ? 2 : (k3 == kEmptyKey ? 3 : -1)));
-          if (e >= 0) {
-            if (*vfill >= fill_limit) { hit_limit = true; break; }  // a new group for a full slice: deferred
-            const unsigned long long old = atomicCAS((unsigned long long*)(skeys + 4 * lb + e), (unsigned long long)kEmptyKey, (unsigned long long)key);
-            if (old == kEmptyKey) { atomicAdd(&s_fill, 1u); slot = 4 * lb + e; break; }
-            if (old == key) { slot = 4 * lb + e; break; }
-            continue;  // another key took the slot: look at this bucket again (it has one EMPTY slot less)
-          }
-          if (++lb == nbs) break;  // the probe leaves the slice
-          ++probes;
-        }
+    for (int r = 0; r < RPT; ++r) {
+      const int i = threadIdx.x + r * kSliceBlock;
+      key[r] = i < m ? stage_row_key<B>(p, st, i) : kEmptyKey;
+      lb[r] = 0;
+      kb[r].x = kb[r].y = kb[r].z = kb[r].w = 0;
+      if (i < m && key[r] != kEmptyKey) {
+        probe |= 1u << r;
+        lb[r] = (int64_t)(agg_hash_u64(key[r]) & nb_mask) - (int64_t)blockIdx.x * nbs;
+        kb[r] = lds_bucket(skeys + 4 * lb[r]);
       }
-      const bool defer = live && slot < 0;
+    }
+    int64_t slot[RPT];
+#pragma unroll
+    for (int r = 0; r < RPT; ++r) {
+      slot[r] = -1;
+      if (!((probe >> r) & 1)) continue;
+      const int mt = bucket_match(kb[r], key[r]);
+      if (mt >= 0) {
+        slot[r] = 4 * lb[r] + mt;
+      } else {
+        slot[r] = slice_probe(skeys, key[r], lb[r], kb[r], nbs, max_probes, &s_fill, fill_limit);
+        if (slot[r] == -2) { hit_limit = true; slot[r] = -1; }
+      }
+    }
+    // the deferred rows (live, no slot), reserved once per warp and row position
+#pragma unroll
+    for (int r = 0; r < RPT; ++r) {
+      const int i = threadIdx.x + r * kSliceBlock;
+      const bool defer = i < m && slot[r] < 0;
       const unsigned dm = __ballot_sync(0xffffffffu, defer);
       if (dm) {
         unsigned long long d = 0;
@@ -1021,29 +1143,50 @@ __global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_
         d = __shfl_sync(0xffffffffu, d, 0) + __popc(dm & ((1u << lane) - 1));
         if (defer) {
 #pragma unroll
-          for (int s = 0; s < NS; ++s) si.deferred[s][d] = vals[s].v[j];
+          for (int s = 0; s < NS; ++s) si.deferred[s][d] = st[(size_t)s * B + i];
         }
       }
-      if (slot < 0) continue;
-      uint64_t* w = sst + slot * nw;
-      for (int u = 0; u < p.n_updates; ++u) {
-        const UpdateDev ud = p.upd[u];
-        hot_update(ud.op, w + ud.word, pick<NS>(vals, ud.slot, j), true);
-      }
     }
+    // phase 2: the updates, each one for all of the thread's rows
+    uint32_t on = 0;
 #pragma unroll
-    for (int s = 0; s < NS; ++s) vals[s] = next[s];
+    for (int r = 0; r < RPT; ++r)
+      if (slot[r] >= 0) on |= 1u << r;
+    PLN_UNROLL
+    for (int u = 0; u < PLN(n_updates); ++u) {
+      const UpdateDev ud = PLN(upd[u]);
+      uint64_t v[RPT];
+      uint64_t* w[RPT];
+#pragma unroll
+      for (int r = 0; r < RPT; ++r) {
+        const bool has = (on >> r) & 1;
+        v[r] = has ? st[(size_t)ud.slot * B + threadIdx.x + r * kSliceBlock] : 0;
+        w[r] = sst + (has ? slot[r] : 0) * nw + ud.word;
+      }
+      slice_update<RPT>(ud.op, w, v, on);
+    }
+    __syncthreads();  // every thread is done with this buffer before the copy issued in the next stage overwrites it
   }
   const int any_hit = __syncthreads_or(hit_limit);
-  for (int64_t i = threadIdx.x; i < S; i += kSliceBlock) t.keys[slot0 + i] = skeys[i];
-  for (int64_t e = threadIdx.x; e < S * nw; e += kSliceBlock) {
-    const int64_t i = e / nw;
-    *word_ptr(t, slot0 + i, (int)(e - i * nw)) = sst[e];
-  }
+#pragma unroll 2
+  for (int64_t i = threadIdx.x; i < S / 2; i += kSliceBlock) gkeys[i] = reinterpret_cast<const ulonglong2*>(skeys)[i];
+#pragma unroll 4
+  for (int64_t e = threadIdx.x; e < S * nw / 2; e += kSliceBlock) gst[e] = reinterpret_cast<const ulonglong2*>(sst)[e];
   if (threadIdx.x == 0) {
     if (s_fill > s_fill0) atomicAdd(t.n_groups, (unsigned long long)(s_fill - s_fill0));
     if (any_hit) atomicAdd(si.n_deferred + 1, 1ULL);
   }
+}
+
+#ifndef DBX_JIT  // everything below is compiled offline only
+// the precompiled passes (no NVRTC on the machine, a plan that could not be specialised, DBX_AGG_JIT=0)
+template <int NS>
+__global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ PartitionOut po) {
+  filter_partition_body<NS>(p, po);
+}
+template <int NS>
+__global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ SliceIn si) {
+  slice_agg_body<NS>(p, si);
 }
 
 // ---------------------------------------------------------------- fused kernel, ring variant

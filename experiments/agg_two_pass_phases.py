@@ -1,6 +1,6 @@
 """Times the phases of the two-pass aggregation of configs[1] (filter v % 3 = 0, sum / count / avg GROUP BY k)
-separately: pass 1 (filter_partition_kernel), pass 2 (slice_agg_kernel, or the fused kernel per L2 region for
-tables with too many slices) and the deferred rows (the fused kernel over a row list), each against its byte
+separately: pass 1 (filter_partition_kernel, or its build for the plan dbx_jit_agg_part), pass 2 (slice_agg_kernel or
+dbx_jit_agg_slice, or the fused kernel per L2 region for tables with too many slices) and the deferred rows (the fused kernel over a row list), each against its byte
 floor at the data-sheet HBM bandwidth.  Kernel times come from torch.profiler (CUDA activities) over `steps`
 queries after one warm-up query; the card's name and power limit are printed with them.
 usage: python experiments/agg_two_pass_phases.py [rows] [n_keys] [steps]"""
@@ -69,9 +69,9 @@ ms = collections.defaultdict(float)
 for e in prof.events():
     if e.device_type == torch.autograd.DeviceType.CUDA:
         name = e.name
-        if "filter_partition_kernel" in name:
+        if "filter_partition_kernel" in name or "dbx_jit_agg_part" in name:
             key = "pass1 filter_partition_kernel"
-        elif "slice_agg_kernel" in name:
+        elif "slice_agg_kernel" in name or "dbx_jit_agg_slice" in name:
             key = "pass2 slice_agg_kernel"
         elif "filter_group_agg_kernel" in name and "true" in name.split(",")[2]:
             key = "deferred rows (fused kernel, row list)"

@@ -143,6 +143,49 @@ class JoinParams(C.Structure):
     ]
 
 
+RF_MAX_INLIST = 4096
+
+
+class RuntimeFilterParams(C.Structure):
+    _fields_ = [
+        ("enable_inlist", C.c_int32),
+        ("enable_bloom", C.c_int32),
+        ("enable_min_max", C.c_int32),
+        ("in_probe", C.c_int32),
+        ("inlist_threshold", C.c_int64),
+        ("bloom_threshold", C.c_int64),
+        ("min_max_threshold", C.c_uint64),
+        ("build_table_rows", C.c_int64),
+        ("selectivity_threshold", C.c_uint64),
+    ]
+
+
+class RfPartInfo(C.Structure):
+    _fields_ = [
+        ("has_min_max", C.c_int32),
+        ("has_inlist", C.c_int32),
+        ("has_bloom", C.c_int32),
+        ("key_dtype", C.c_int32),
+        ("min", Scalar),
+        ("max", Scalar),
+        ("inlist_len", C.c_int64),
+        ("bloom_bytes", C.c_int64),
+    ]
+
+
+class RfInfo(C.Structure):
+    _fields_ = [
+        ("n_parts", C.c_int32),
+        ("in_probe", C.c_int32),
+        ("build_rows", C.c_int64),
+        ("apply_rows_checked", C.c_int64),
+        ("apply_rows_rejected", C.c_int64),
+        ("probe_rows_checked", C.c_int64),
+        ("probe_rows_rejected", C.c_int64),
+        ("parts", RfPartInfo * MAX_JOIN_KEYS),
+    ]
+
+
 EXPR_COLUMN, EXPR_CONST, EXPR_CAST, EXPR_CALL = 0, 1, 2, 3
 (FN_PLUS, FN_MINUS, FN_MULTIPLY, FN_DIVIDE, FN_DIV, FN_MODULO, FN_NEGATE, FN_EQ, FN_NOTEQ, FN_LT, FN_LTE, FN_GT, FN_GTE, FN_AND, FN_OR, FN_NOT,
  FN_IS_NULL, FN_IS_NOT_NULL) = range(18)
@@ -176,4 +219,6 @@ EXPORTS = [
     "dbx_block_take", "dbx_block_take_ranges", "dbx_block_scatter", "dbx_block_concat",
     "dbx_eval_scalar", "dbx_op_kernel_variant", "dbx_agg_jit_selftest", "dbx_eval_jit_selftest",
     "dbx_agg_partial_serialize", "dbx_agg_final_merge_serialized",
+    "dbx_join_runtime_filter", "dbx_runtime_filter_info", "dbx_runtime_filter_export", "dbx_runtime_filter_apply",
+    "dbx_runtime_filter_destroy",
 ]

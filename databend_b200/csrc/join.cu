@@ -34,6 +34,7 @@
 
 #include "plan.h"
 #include "runtime.h"
+#include "runtime_filter.cuh"
 
 namespace dbx {
 
@@ -130,6 +131,8 @@ struct JoinProbeParams {
   unsigned long long* cursor;  // number of matches (may exceed out_cap: then the host retries)
   uint8_t* matched;            // build-side kinds: one byte per build row, set when a probe row matches it
   JoinKeyPack pack;            // composite keys (PACKED kernels): the probe key columns
+  RfPartDev rf;                // RF kernels: the runtime filter's min-max and bloom (runtime_filter.cuh)
+  unsigned long long* rf_rejected;  // RF kernels: rows the filter turned away
 };
 
 __device__ __forceinline__ uint64_t load_key(const DevCol& c, int64_t row) {
@@ -368,7 +371,10 @@ __global__ void join_dup_check_kernel(const __grid_constant__ JoinTableDev t, un
 // NULL in any key column is a miss.  The PACKED instantiations ask for three resident blocks per
 // SM: without a minimum ptxas caps them near 64 registers and spills, with one it takes up to 94
 // registers (two blocks per SM), and the probe is bound by latency, so occupancy counts.
-template <int KW, bool PACKED, bool UNIQUE, bool MARK>
+// RF (single key): the join's runtime filter tests min-max and bloom before the table walk; a
+// rejected row cannot match and takes the no-match path, which is right for every kind.  The
+// RF = false instantiations compile to the code as it was before runtime filters.
+template <int KW, bool PACKED, bool UNIQUE, bool MARK, bool RF = false>
 __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
   __shared__ unsigned int s_warp[kJoinBlock / 32];
   __shared__ unsigned long long s_base;
@@ -378,6 +384,7 @@ __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel
   const int64_t n_iter = (p.n_rows + step - 1) / step;
   const int64_t row_end = p.row_begin + p.n_rows;
   const JEntry<KW>* const entries = (const JEntry<KW>*)p.table.entries;
+  unsigned int rf_rej = 0;
   for (int64_t it = 0; it < n_iter; ++it) {
     int64_t r[2];
     r[0] = p.row_begin + it * step + (int64_t)blockIdx.x * blockDim.x * 2 + threadIdx.x;
@@ -393,6 +400,10 @@ __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel
       in_range[j] = r[j] < row_end;
       if (PACKED) go[j] = in_range[j] && load_packed_key<KW>(p.pack, r[j], k[j], kh[j]);
       else go[j] = in_range[j] && !(p.key.validity && !bit_test(p.key.validity, p.key.vbit_off + r[j]));
+      if (RF && go[j]) {
+        const uint64_t v = load_key(p.key, r[j]);
+        if (!rf_min_max_pass(p.rf, v) || !rf_bloom_pass(p.rf, v)) { go[j] = false; ++rf_rej; }
+      }
       if (go[j]) {
         if (!PACKED) k[j] = load_key(p.key, r[j]);
         b0[j] = join_home<KW>(p.table, k[j], &rb[j], kh[j]);
@@ -474,6 +485,10 @@ __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel
         }
       }
     }
+  }
+  if (RF) {  // RuntimeFilterStats: one atomic per warp
+    const unsigned int w = __reduce_add_sync(0xffffffffu, rf_rej);
+    if (lane == 0 && w) atomicAdd(p.rf_rejected, (unsigned long long)w);
   }
 }
 
@@ -601,6 +616,7 @@ class JoinOp : public Op {
   std::vector<std::unique_ptr<OwnedBlock>> outputs;  // joined blocks waiting to be pulled (device resident)
   size_t next_out = 0;
   DevBuf matched;             // build-side kinds: one byte per build row, 1 once any probe row matched it
+  std::shared_ptr<RfData> rf_probe;  // runtime filter the probe kernel tests (single key), shared with its handle
   bool final_probed = false;  // Join::final_probe ran: no more probe blocks until reset
   // key pairs (1 + n_extra_keys); packed: composite key of key_words words, fields in *_part
   int n_keys = 1, key_words = 1;
@@ -829,14 +845,14 @@ class JoinOp : public Op {
     return DBX_OK;
   }
 
-  template <int KW, bool PACKED>
+  template <int KW, bool PACKED, bool RF = false>
   void launch_probe2(const JoinProbeParams& pp, int grid) {
     if (pp.matched) {
-      if (build_unique) join_probe2_kernel<KW, PACKED, true, true><<<grid, kJoinBlock, 0, stream>>>(pp);
-      else join_probe2_kernel<KW, PACKED, false, true><<<grid, kJoinBlock, 0, stream>>>(pp);
+      if (build_unique) join_probe2_kernel<KW, PACKED, true, true, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<KW, PACKED, false, true, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
     } else {
-      if (build_unique) join_probe2_kernel<KW, PACKED, true, false><<<grid, kJoinBlock, 0, stream>>>(pp);
-      else join_probe2_kernel<KW, PACKED, false, false><<<grid, kJoinBlock, 0, stream>>>(pp);
+      if (build_unique) join_probe2_kernel<KW, PACKED, true, false, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<KW, PACKED, false, false, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
     }
   }
   void launch_probe(const JoinProbeParams& pp, int64_t rows) {
@@ -849,6 +865,7 @@ class JoinOp : public Op {
       else launch_probe2<1, true>(pp, grid);
       return;
     }
+    if (rf_probe) { launch_probe2<1, false, true>(pp, grid); return; }
     if (old_probe && !pp.matched) { join_probe_kernel<<<grid_rows(rows), kJoinBlock, 0, stream>>>(pp); return; }
     launch_probe2<1, false>(pp, grid);
   }
@@ -860,6 +877,7 @@ class JoinOp : public Op {
     if (b->num_cols != n_probe_cols) { err.set("probe_block: block does not match the probe schema"); return DBX_ERR_INVALID; }
     const int64_t n = b->num_rows;
     if (n == 0) return DBX_OK;
+    if (rf_probe) rf_probe->probe_checked += n;
     DevCol cols[kMaxJoinCols];
     DBX_TRY(stager.begin());
     for (int c = 0; c < n_probe_cols; ++c) {
@@ -903,6 +921,10 @@ class JoinOp : public Op {
       pp.out_cap = out_cap;
       pp.cursor = (unsigned long long*)cursor.p;
       pp.matched = build_side_kind(prm.kind) ? (uint8_t*)matched.p : nullptr;
+      if (rf_probe) {  // a retried probe must not count its rejections twice
+        pp.rf = rf_probe->parts[0].dev();
+        pp.rf_rejected = attempt == 0 ? (unsigned long long*)rf_probe->probe_rejected.p : (unsigned long long*)cursor.p + 4;
+      }
       if (packed) {
         pp.pack.n = n_keys;
         for (int i = 0; i < n_keys; ++i) {
@@ -1109,7 +1131,42 @@ class JoinOp : public Op {
     return fill_owned_block(hb.release(), out);
   }
 
+  // Join runtime filter (runtime_filter.cu) of the finished build side; in_probe also hands it to the
+  // probe kernel until reset
+  int32_t runtime_filter(const dbx_runtime_filter_params* p, dbx_runtime_filter** out) {
+    const int k = prm.kind;
+    if (k == DBX_JOIN_LEFT || k == DBX_JOIN_LEFT_ANTI || k == DBX_JOIN_FULL) {
+      err.set("runtime filter: LEFT, LEFT ANTI and FULL joins keep every probe row, so no filter is built for them");
+      return DBX_ERR_UNSUPPORTED;
+    }
+    if (!finished) { err.set("runtime filter before final_build"); return DBX_ERR_STATE; }
+    if (p->in_probe && packed) { err.set("runtime filter: in_probe is built for single-key joins only (apply the filter to probe blocks instead)"); return DBX_ERR_UNSUPPORTED; }
+    RfBuildKey keys[DBX_MAX_JOIN_KEYS];
+    for (int i = 0; i < n_keys; ++i) {
+      const GrowCol& g = build[key_build_col[i]];
+      keys[i] = RfBuildKey{g.data.p, g.nullable ? (const uint8_t*)g.valid_bytes.p : nullptr, build_dtype[key_build_col[i]],
+                           probe_dtype[key_probe_col[i]]};
+    }
+    std::shared_ptr<RfData> d;
+    DBX_TRY(build_runtime_filter(err, stream, device, *p, keys, n_keys, build_rows, &d));
+    drop_runtime_filter();
+    if (p->in_probe && (d->parts[0].has_min_max || d->parts[0].has_bloom)) {
+      rf_probe = d;
+      d->in_probe = true;
+    }
+    *out = make_runtime_filter_handle(std::move(d));
+    if (!*out) { drop_runtime_filter(); err.set("runtime filter: could not create the handle's stream"); return DBX_ERR_CUDA; }
+    return DBX_OK;
+  }
+  void drop_runtime_filter() {
+    if (rf_probe) rf_probe->in_probe = false;
+    rf_probe.reset();
+  }
+  ~JoinOp() override { drop_runtime_filter(); }
+  const char* kernel_variant() override { return rf_probe ? "precompiled kernels; runtime filter in the probe" : Op::kernel_variant(); }
+
   int32_t reset() override {
+    drop_runtime_filter();
     build_rows = 0;
     final_probed = false;  // the matched map is cleared by the next final_build
     outputs.clear();
@@ -1143,4 +1200,15 @@ extern "C" int32_t dbx_join_final_probe(dbx_op* op) {
   if (o->kind != DBX_OP_JOIN) { o->err.set("dbx_join_final_probe: not a join operator"); return DBX_ERR_INVALID; }
   DBX_CUDA_TRY(o->err, cudaSetDevice(o->device));
   return static_cast<JoinOp*>(o)->final_probe();
+}
+
+extern "C" int32_t dbx_join_runtime_filter(dbx_op* op, const dbx_runtime_filter_params* params, dbx_runtime_filter** out) {
+  if (!op || !params || !out) { g_create_error.set("dbx_join_runtime_filter: null argument"); return DBX_ERR_INVALID; }
+  *out = nullptr;
+  Op* o = reinterpret_cast<Op*>(op);
+  if (o->kind != DBX_OP_JOIN) { o->err.set("dbx_join_runtime_filter: not a join operator"); g_create_error.set(o->err.msg); return DBX_ERR_INVALID; }
+  DBX_CUDA_TRY(o->err, cudaSetDevice(o->device));
+  const int32_t st = static_cast<JoinOp*>(o)->runtime_filter(params, out);
+  if (st != DBX_OK) g_create_error.set(o->err.msg);
+  return st;
 }

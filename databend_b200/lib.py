@@ -104,6 +104,11 @@ def load():
         "dbx_block_scatter": (i32, [i32, P(abi.Block), vp, i32, i32, i32, P(abi.Block)]),
         "dbx_block_concat": (i32, [i32, P(abi.Block), i32, i32, P(abi.Block)]),
         "dbx_eval_scalar": (i32, [i32, P(abi.Expr), P(abi.Block), i32, P(abi.Block), P(i32), P(i64)]),
+        "dbx_join_runtime_filter": (i32, [vp, P(abi.RuntimeFilterParams), P(vp)]),
+        "dbx_runtime_filter_info": (i32, [vp, P(abi.RfInfo)]),
+        "dbx_runtime_filter_export": (i32, [vp, i32, P(C.c_uint32), i64, P(i64), i64]),
+        "dbx_runtime_filter_apply": (i32, [vp, P(abi.Block), P(i32), i32, P(abi.Block), P(i64)]),
+        "dbx_runtime_filter_destroy": (i32, [vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)  # AttributeError = the library does not export a declared symbol

@@ -409,6 +409,21 @@ class HashJoin(_Op):
             out.append(_block_from_c(ob, self.device) if out_mem == abi.MEM_HOST else ob)
         return out
 
+    def runtime_filter(self, enable_inlist: bool = True, enable_bloom: bool = True, enable_min_max: bool = True,
+                       in_probe: bool = False, inlist_threshold: int = 1024, bloom_threshold: int = 3_000_000,
+                       min_max_threshold: int = 2**64 - 1, build_table_rows: int = 0,
+                       selectivity_threshold: int = 10) -> RuntimeFilter:
+        """The runtime filter of the finished build side (defaults = the reference's settings).
+        build_table_rows = 0 means unknown, so no bloom.  in_probe: the probe kernel also tests min-max
+        and bloom until reset() (single-key joins)."""
+        p = abi.RuntimeFilterParams()
+        p.enable_inlist, p.enable_bloom, p.enable_min_max, p.in_probe = int(enable_inlist), int(enable_bloom), int(enable_min_max), int(in_probe)
+        p.inlist_threshold, p.bloom_threshold, p.min_max_threshold = inlist_threshold, bloom_threshold, min_max_threshold
+        p.build_table_rows, p.selectivity_threshold = build_table_rows, selectivity_threshold
+        h = C.c_void_p()
+        check(load().dbx_join_runtime_filter(self._h, C.byref(p), C.byref(h)), self._h)
+        return RuntimeFilter(h, self.device)
+
     def final_probe(self, out_mem: int = abi.MEM_HOST) -> List[DataBlock]:
         """Join::final_probe, called once after the last probe_block: the build rows that RIGHT,
         RIGHT ANTI and FULL keep unmatched, or that RIGHT SEMI matched (each once).  Empty for the
@@ -421,6 +436,95 @@ class HashJoin(_Op):
                 break
             out.append(_block_from_c(ob, self.device) if out_mem == abi.MEM_HOST else ob)
         return out
+
+
+@dataclass
+class RuntimeFilterPartInfo:
+    """One key pair's filters: which exist, the bounds and sizes (common type `key_dtype`)."""
+    has_min_max: bool
+    has_inlist: bool
+    has_bloom: bool
+    key_dtype: int
+    min: Optional[int]
+    max: Optional[int]
+    inlist_len: int
+    bloom_bytes: int
+
+
+@dataclass
+class RuntimeFilterInfo:
+    """RuntimeFilterInfo + RuntimeFilterStats (catalog/src/runtime_filter_info.rs)."""
+    build_rows: int
+    in_probe: bool
+    apply_rows_checked: int
+    apply_rows_rejected: int
+    probe_rows_checked: int
+    probe_rows_rejected: int
+    parts: List[RuntimeFilterPartInfo]
+
+
+class RuntimeFilter:
+    """A join's runtime filter (dbx_runtime_filter): min-max, IN-list and bloom per key pair, built on
+    the device from the build keys.  Valid after the join is reset or closed."""
+
+    def __init__(self, handle: C.c_void_p, device: int):
+        self._h, self.device = handle, device
+
+    def info(self) -> RuntimeFilterInfo:
+        r = abi.RfInfo()
+        check(load().dbx_runtime_filter_info(self._h, C.byref(r)))
+        parts = []
+        for i in range(r.n_parts):
+            pi = r.parts[i]
+            signed = pi.key_dtype in _SIGNED
+
+            def val(s):
+                return None if s.is_null else (s.v.i64 if signed else s.v.u64)
+            parts.append(RuntimeFilterPartInfo(bool(pi.has_min_max), bool(pi.has_inlist), bool(pi.has_bloom), pi.key_dtype,
+                                               val(pi.min), val(pi.max), pi.inlist_len, pi.bloom_bytes))
+        return RuntimeFilterInfo(r.build_rows, bool(r.in_probe), r.apply_rows_checked, r.apply_rows_rejected,
+                                 r.probe_rows_checked, r.probe_rows_rejected, parts)
+
+    def bloom_words(self, part: int = 0) -> np.ndarray:
+        """The bloom filter of key pair `part` as uint32 words (8 per 32-byte block); empty if none."""
+        n = self.info().parts[part].bloom_bytes // 4
+        out = np.zeros(n, dtype=np.uint32)
+        if n:
+            check(load().dbx_runtime_filter_export(self._h, part, out.ctypes.data_as(C.POINTER(C.c_uint32)), n, None, 0))
+        return out
+
+    def inlist(self, part: int = 0) -> np.ndarray:
+        """The distinct build keys of pair `part`, ascending, as the common type (empty if none)."""
+        pi = self.info().parts[part]
+        out = np.zeros(pi.inlist_len, dtype=np.int64)
+        if pi.inlist_len:
+            check(load().dbx_runtime_filter_export(self._h, part, None, 0, out.ctypes.data_as(C.POINTER(C.c_int64)), pi.inlist_len))
+        return out.view(np_dtype(abi.I64 if pi.key_dtype in _SIGNED else abi.U64)).astype(np_dtype(pi.key_dtype))
+
+    def apply(self, block: DataBlock, key_cols: Union[int, Sequence[int]]) -> Column:
+        """ExprBloomFilter::apply ANDed over the parts: a Boolean column, true where the probe row may
+        match.  key_cols: the probe key column of each key pair in `block`."""
+        cols = _key_list(key_cols)
+        kc = (C.c_int32 * len(cols))(*cols)
+        b, keep = block.as_c()
+        out = abi.Block()
+        passed = C.c_int64(0)
+        check(load().dbx_runtime_filter_apply(self._h, C.byref(b), kc, abi.MEM_HOST, C.byref(out), C.byref(passed)))
+        del keep
+        col = _block_from_c(out, self.device).columns[0]
+        self.last_passed = passed.value
+        return col
+
+    def close(self):
+        if self._h:
+            load().dbx_runtime_filter_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def filter_group_aggregate(blocks: Sequence[DataBlock], params: AggregatorParams, filter_expr: Optional[E.Node] = None,

@@ -317,6 +317,79 @@ int32_t dbx_join_probe(dbx_op* op, const dbx_block* block);
  * returns DBX_ERR_STATE until dbx_op_reset. */
 int32_t dbx_join_final_probe(dbx_op* op);
 
+/* Join runtime filters (hash_join/runtime_filter/local_builder.rs:86-167, convert.rs:50-117,
+ * catalog/src/sbbf.rs): after Join::final_build, summarise the build keys as a min-max range, an
+ * IN-list of the distinct keys and a split-block bloom filter, then drop probe rows that cannot
+ * match before the join touches its table.  Built for INNER, LEFT SEMI, RIGHT, RIGHT SEMI and RIGHT
+ * ANTI (physical_plans/runtime_filter/builder.rs:66-76); LEFT, LEFT ANTI and FULL keep every probe
+ * row, so they are refused with DBX_ERR_UNSUPPORTED.  One part per key pair; a composite key's
+ * parts are ANDed.  Each part works on the pair's common type (the join's key rule): min, max and
+ * the IN-list values are the keys converted to it, the bloom hashes its bits zero-extended to 64
+ * (KeysU8/U16/U32/U64 + murmur3 fmix64).  NULL build keys never match and are left out of all three
+ * filters; a NULL probe key is rejected.
+ *   - min-max: built while build_rows <= min_max_threshold;
+ *   - IN-list: the sorted distinct keys, built while build_rows <= inlist_threshold (at most
+ *     DBX_RF_MAX_INLIST);
+ *   - bloom: built while build_rows <= bloom_threshold and build_table_rows is known (> 0) and
+ *     build_rows / build_table_rows * 100 < selectivity_threshold (builder.rs:17-57).  Sized from the
+ *     non-NULL build keys with fpp 0.01 (sbbf.rs:225-262).
+ * An empty build side carries no filters.  in_probe = 1 also hands min-max and bloom to the join's
+ * probe kernel, which turns rejected rows onto its no-match path (single-key joins only; composite
+ * keys use dbx_runtime_filter_apply, in_probe is refused with DBX_ERR_UNSUPPORTED).  The join drops
+ * that filter on dbx_op_reset or on the next dbx_join_runtime_filter call.  The handle stays valid
+ * after the join is reset or destroyed, and destroying it while the join still probes with it is
+ * safe.  Errors of the runtime-filter calls are read with dbx_last_error(NULL). */
+#define DBX_RF_MAX_INLIST 4096
+typedef struct dbx_runtime_filter_params {
+  int32_t enable_inlist;          /* enable_inlist_runtime_filter */
+  int32_t enable_bloom;           /* enable_bloom_runtime_filter */
+  int32_t enable_min_max;         /* enable_min_max_runtime_filter */
+  int32_t in_probe;               /* 1: the probe kernel tests min-max and bloom itself */
+  int64_t inlist_threshold;       /* inlist_runtime_filter_threshold (1024), 0 .. DBX_RF_MAX_INLIST */
+  int64_t bloom_threshold;        /* bloom_runtime_filter_threshold (3000000) */
+  uint64_t min_max_threshold;     /* min_max_runtime_filter_threshold (UINT64_MAX) */
+  int64_t build_table_rows;       /* rows of the build side's table; 0 = unknown: no bloom */
+  uint64_t selectivity_threshold; /* join_runtime_filter_selectivity_threshold, percent (10) */
+} dbx_runtime_filter_params;
+
+typedef struct dbx_runtime_filter dbx_runtime_filter; /* opaque */
+
+typedef struct dbx_rf_part_info {
+  int32_t has_min_max, has_inlist, has_bloom;
+  int32_t key_dtype;              /* the pair's common type (dbx_dtype) */
+  dbx_scalar min, max;            /* in key_dtype; is_null when no build key is non-NULL */
+  int64_t inlist_len;             /* distinct non-NULL build keys */
+  int64_t bloom_bytes;            /* 32 .. 128 MiB, a power of two */
+} dbx_rf_part_info;
+
+/* RuntimeFilterInfo + RuntimeFilterStats.  checked / rejected count probe rows: apply counts every
+ * row of a block and rejects NULL keys too; the probe counts every row of a block and rejects the
+ * non-NULL keys the filter turned away. */
+typedef struct dbx_rf_info {
+  int32_t n_parts;                /* key pairs */
+  int32_t in_probe;               /* the join still probes with this filter */
+  int64_t build_rows;             /* build rows the filter was built from, NULL keys included */
+  int64_t apply_rows_checked, apply_rows_rejected;
+  int64_t probe_rows_checked, probe_rows_rejected;
+  dbx_rf_part_info parts[DBX_MAX_JOIN_KEYS];
+} dbx_rf_info;
+
+/* Build the runtime filter of a finished join (after dbx_op_finish; DBX_ERR_STATE before). */
+int32_t dbx_join_runtime_filter(dbx_op* op, const dbx_runtime_filter_params* params, dbx_runtime_filter** out);
+int32_t dbx_runtime_filter_info(dbx_runtime_filter* rf, dbx_rf_info* out);
+/* Copy part `part`'s bloom words (bloom_bytes / 4 uint32, block after block) and IN-list (inlist_len
+ * values in ascending order of the common type, each widened to 64 bits) into host buffers; either
+ * pointer may be NULL.  A buffer that is too small is DBX_ERR_INVALID. */
+int32_t dbx_runtime_filter_export(dbx_runtime_filter* rf, int32_t part, uint32_t* bloom_words, int64_t bloom_cap,
+                                  int64_t* inlist, int64_t inlist_cap);
+/* ExprBloomFilter::apply (storages/fuse/src/pruning/expr_bloom_filter.rs:31-44) ANDed over parts and
+ * filters: out = a library-owned block with ONE DBX_BOOL column (bit-packed, LSB first, bit offset 0),
+ * true where the row may match.  key_cols[i] is the probe key column of pair i in `block` (its dtype
+ * must be the join's probe key dtype).  *n_passed = rows set (may be NULL). */
+int32_t dbx_runtime_filter_apply(dbx_runtime_filter* rf, const dbx_block* block, const int32_t* key_cols, int32_t out_mem,
+                                 dbx_block* out, int64_t* n_passed);
+int32_t dbx_runtime_filter_destroy(dbx_runtime_filter* rf);
+
 /* AGG_FINAL input: hand over a partial operator's device-resident payload
  * (AggregateMeta::AggregatePayload, aggregate_meta.rs) without leaving HBM. */
 int32_t dbx_agg_final_merge_partial(dbx_op* final_op, dbx_op* partial_op);

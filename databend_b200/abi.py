@@ -190,6 +190,7 @@ EXPR_COLUMN, EXPR_CONST, EXPR_CAST, EXPR_CALL = 0, 1, 2, 3
 (FN_PLUS, FN_MINUS, FN_MULTIPLY, FN_DIVIDE, FN_DIV, FN_MODULO, FN_NEGATE, FN_EQ, FN_NOTEQ, FN_LT, FN_LTE, FN_GT, FN_GTE, FN_AND, FN_OR, FN_NOT,
  FN_IS_NULL, FN_IS_NOT_NULL) = range(18)
 MAX_EXPR_NODES = 32
+MAX_COMPUTED_COLS = 4
 
 
 class ExprNode(C.Structure):
@@ -220,5 +221,5 @@ EXPORTS = [
     "dbx_eval_scalar", "dbx_op_kernel_variant", "dbx_agg_jit_selftest", "dbx_eval_jit_selftest",
     "dbx_agg_partial_serialize", "dbx_agg_final_merge_serialized",
     "dbx_join_runtime_filter", "dbx_runtime_filter_info", "dbx_runtime_filter_export", "dbx_runtime_filter_apply",
-    "dbx_runtime_filter_destroy",
+    "dbx_runtime_filter_destroy", "dbx_op_create_computed", "dbx_agg_expr_jit_selftest",
 ]

@@ -35,14 +35,31 @@ inline int grid_for_entries(int64_t n) {
 }
 
 // ---------------------------------------------------------------- plan
+constexpr int kMaxCols = 64 + kMaxComputed;  // input columns, then computed columns
+
 struct AggPlan {
   dbx_agg_params params;
-  int n_cols = 0;
-  int col_dtype[64];
-  bool col_nullable[64];
+  int n_cols = 0;   // input columns (the pushed blocks' schema)
+  int n_comp = 0;   // computed columns: column n_cols + i is computed[i]
+  int col_dtype[kMaxCols];
+  bool col_nullable[kMaxCols];
 
   int n_slots = 0;
-  int slot_col[kMaxSlots];
+  // input column loaded into each slot; -1: the slot holds a computed value only.  While the plan is
+  // built with computed columns these are virtual slots (one per column, computed ones included), mapped
+  // onto at most kMaxSlots by allocate_slots.
+  int slot_col[kMaxCols];
+  // computed columns: the type-checked programs (COLUMN nodes name input columns), and what the
+  // kernels evaluate after allocate_slots (only the computed columns the plan uses)
+  NodeDev comp_nodes[kMaxComputed][kMaxExprNodes];
+  int comp_n_nodes[kMaxComputed] = {};
+  bool comp_raises[kMaxComputed] = {};
+  int n_comp_ev = 0, comp_pred = 0, n_cnodes = 0;
+  CompDev comp[kMaxComputed];
+  NodeDev cnodes[kMaxCompNodes];
+  uint32_t fresh_slots = 0;
+  bool comp_nullable = false;  // a computed column the kernels evaluate may be NULL
+  bool can_raise = false;      // a computed column evaluated after the predicate can raise: errors are recorded
 
   int n_nodes = 0;
   PredNodeDev nodes[DBX_MAX_PRED_NODES];
@@ -78,7 +95,7 @@ struct AggPlan {
   int slot_of(int col, ErrorSink* err) {
     for (int s = 0; s < n_slots; ++s)
       if (slot_col[s] == col) return s;
-    if (n_slots == kMaxSlots) { err->set("operator reads more than 8 distinct columns"); return -1; }
+    if (n_slots == (n_comp ? kMaxCols : kMaxSlots)) { err->set("operator reads more than 8 distinct columns"); return -1; }
     slot_col[n_slots] = col;
     return n_slots++;
   }
@@ -145,7 +162,7 @@ int32_t lower_cmp(AggPlan* pl, const dbx_pred_node& in, PredNodeDev* out, ErrorS
     return DBX_OK;
   }
   if (l.is_const) { std::swap(l, r); cmp = flip_cmp(cmp); }
-  if (l.col < 0 || l.col >= pl->n_cols) { err->set("predicate references a column outside the input schema"); return DBX_ERR_INVALID; }
+  if (l.col < 0 || l.col >= pl->n_cols + pl->n_comp) { err->set("predicate references a column outside the input schema"); return DBX_ERR_INVALID; }
   if (!r.is_const && r.arith != DBX_ARITH_NONE) { err->set("arithmetic on the right-hand column of a comparison is not supported"); return DBX_ERR_UNSUPPORTED; }
   int lcls = loaded_class(pl->col_dtype[l.col]);
   out->l_slot = pl->slot_of(l.col, err);
@@ -174,7 +191,7 @@ int32_t lower_cmp(AggPlan* pl, const dbx_pred_node& in, PredNodeDev* out, ErrorS
     return DBX_ERR_INVALID;
   }
   if (!r.is_const) {
-    if (r.col < 0 || r.col >= pl->n_cols) { err->set("predicate references a column outside the input schema"); return DBX_ERR_INVALID; }
+    if (r.col < 0 || r.col >= pl->n_cols + pl->n_comp) { err->set("predicate references a column outside the input schema"); return DBX_ERR_INVALID; }
     int rcls = loaded_class(pl->col_dtype[r.col]);
     if (rcls != lcls) { err->set("comparison between columns of different numeric classes is not supported"); return DBX_ERR_UNSUPPORTED; }
     out->r_slot = pl->slot_of(r.col, err);
@@ -238,7 +255,7 @@ int32_t lower_predicate(AggPlan* pl, const dbx_predicate& pred, ErrorSink* err) 
       case DBX_PRED_BOOLCOL:
         memset(out, 0, sizeof(*out));
         out->kind = DBX_PRED_BOOLCOL;
-        if (in.value < 0 || in.value >= pl->n_cols || pl->col_dtype[in.value] != DBX_BOOL) { err->set("predicate: BooleanColumn must reference a Boolean column"); return DBX_ERR_INVALID; }
+        if (in.value < 0 || in.value >= pl->n_cols + pl->n_comp || pl->col_dtype[in.value] != DBX_BOOL) { err->set("predicate: BooleanColumn must reference a Boolean column"); return DBX_ERR_INVALID; }
         out->value = pl->slot_of(in.value, err);
         if (out->value < 0) return DBX_ERR_UNSUPPORTED;
         depth += 1;
@@ -257,7 +274,158 @@ int32_t lower_predicate(AggPlan* pl, const dbx_predicate& pred, ErrorSink* err) 
   return DBX_OK;
 }
 
-int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols, AggPlan* pl, ErrorSink* err) {
+// Type-checks the computed columns (dbx_eval_scalar's inference over the input schema) and appends
+// them to the plan's columns.
+int32_t add_computed(AggPlan* pl, const dbx_expr* comp, int n_comp, ErrorSink* err) {
+  if (n_comp < 0 || n_comp > kMaxComputed) { err->set("computed columns: n_computed outside 0 .. DBX_MAX_COMPUTED_COLS"); return DBX_ERR_INVALID; }
+  if (n_comp > 0 && !comp) { err->set("computed columns: null list"); return DBX_ERR_INVALID; }
+  if (pl->n_cols + n_comp > 64) { err->set("computed columns: more than 64 input and computed columns"); return DBX_ERR_INVALID; }
+  for (int i = 0; i < n_comp; ++i) {
+    const dbx_expr& e = comp[i];
+    for (int k = 0; k < e.n_nodes && k < DBX_MAX_EXPR_NODES; ++k)
+      if (e.nodes[k].kind == DBX_EXPR_COLUMN && e.nodes[k].col >= pl->n_cols && e.nodes[k].col < pl->n_cols + n_comp) {
+        err->set("computed column " + std::to_string(i) + " references a computed column (only input columns may be referenced)");
+        return DBX_ERR_INVALID;
+      }
+    int dt = 0;
+    bool nullable = false;
+    const int32_t st = infer_expr_types(e, pl->n_cols, pl->col_dtype, pl->col_nullable, pl->comp_nodes[i], &dt, &nullable, *err);
+    if (st != DBX_OK) { err->set("computed column " + std::to_string(i) + ": " + err->msg); return st; }
+    pl->comp_n_nodes[i] = e.n_nodes;
+    pl->comp_raises[i] = expr_can_raise(pl->comp_nodes[i], e.n_nodes);
+    pl->col_dtype[pl->n_cols + i] = dt;
+    pl->col_nullable[pl->n_cols + i] = nullable;
+  }
+  pl->n_comp = n_comp;
+  return DBX_OK;
+}
+
+// Maps the plan's virtual slots (one per column it reads) onto at most kMaxSlots.  Per tile the kernels
+// load the inputs, evaluate the computed columns the predicate uses, the predicate, then the other
+// computed columns; a computed column takes the slot of a value whose last use is at or before its own
+// evaluation (an input only the predicate or earlier expressions read), else a new slot.
+int32_t allocate_slots(AggPlan* pl, ErrorSink* err) {
+  const int nv0 = pl->n_slots;
+  bool pred_use[kMaxCols] = {}, late_use[kMaxCols] = {};
+  for (int i = 0; i < pl->n_nodes; ++i) {
+    const PredNodeDev& n = pl->nodes[i];
+    if (n.kind == DBX_PRED_CMP) { pred_use[n.l_slot] = true; if (n.r_slot >= 0) pred_use[n.r_slot] = true; }
+    else if (n.kind == DBX_PRED_BOOLCOL) pred_use[n.value] = true;
+  }
+  if (pl->grouped) {
+    if (pl->n_key_parts > 1) for (int j = 0; j < pl->n_key_parts; ++j) late_use[pl->key_parts[j].slot] = true;
+    else late_use[pl->key_slot] = true;
+  }
+  for (int u = 0; u < pl->n_updates; ++u)
+    if (pl->upd[u].op != UPD_INC) late_use[pl->upd[u].slot] = true;
+  // evaluation order: computed columns the predicate reads, then the others the plan reads
+  int order[kMaxComputed], n_ord = 0, n_pred = 0;
+  for (int phase = 0; phase < 2; ++phase)
+    for (int v = 0; v < nv0; ++v) {
+      const int c = pl->slot_col[v] - pl->n_cols;
+      if (c < 0 || pred_use[v] != (phase == 0)) continue;
+      if (pl->comp_raises[c] && phase == 0) {
+        err->set("computed column " + std::to_string(c) + " is used by the predicate and can raise (division by a column or by zero, an overflowing cast or the negation of a 64-bit integer): "
+                 "which rows reach it would depend on the evaluation order of the filter");
+        return DBX_ERR_UNSUPPORTED;
+      }
+      order[n_ord++] = c;
+      n_pred += phase == 0;
+    }
+  // the inputs of the evaluated computed columns
+  for (int k = 0; k < n_ord; ++k) {
+    const int c = order[k];
+    for (int i = 0; i < pl->comp_n_nodes[c]; ++i)
+      if (pl->comp_nodes[c][i].kind == DBX_EXPR_COLUMN && pl->slot_of(pl->comp_nodes[c][i].col, err) < 0) return DBX_ERR_UNSUPPORTED;
+  }
+  const int nv = pl->n_slots;
+  // positions: 0 load, 1 .. n_pred predicate's computed columns, n_pred + 1 predicate, then the others
+  auto comp_pos = [&](int c) { for (int k = 0; k < n_ord; ++k) if (order[k] == c) return k < n_pred ? 1 + k : 2 + k; return -1; };
+  const int kEnd = 1 << 20;
+  int last[kMaxCols], def[kMaxCols];
+  for (int v = 0; v < nv; ++v) {
+    const int c = pl->slot_col[v] - pl->n_cols;
+    def[v] = c < 0 ? 0 : comp_pos(c);
+    last[v] = late_use[v] ? kEnd : (pred_use[v] ? n_pred + 1 : 0);
+  }
+  for (int k = 0; k < n_ord; ++k) {
+    const int c = order[k];
+    for (int i = 0; i < pl->comp_n_nodes[c]; ++i)
+      if (pl->comp_nodes[c][i].kind == DBX_EXPR_COLUMN) {
+        const int v = pl->slot_of(pl->comp_nodes[c][i].col, err);
+        last[v] = std::max(last[v], comp_pos(c));
+      }
+  }
+  // inputs first (all are live at the load), then the computed columns in evaluation order
+  int phys[kMaxCols], occ_last[kMaxSlots], phys_col[kMaxSlots], n_phys = 0;
+  uint32_t fresh = 0;
+  for (int v = 0; v < nv; ++v) {
+    phys[v] = -1;
+    if (pl->slot_col[v] >= pl->n_cols) continue;
+    if (n_phys == kMaxSlots) break;
+    phys_col[n_phys] = pl->slot_col[v];
+    occ_last[n_phys] = last[v];
+    phys[v] = n_phys++;
+  }
+  for (int k = 0; k < n_ord; ++k) {
+    int v = 0;
+    while (pl->slot_col[v] != pl->n_cols + order[k]) ++v;
+    int s = 0;
+    while (s < n_phys && occ_last[s] > def[v]) ++s;
+    if (s == n_phys) {
+      if (n_phys == kMaxSlots) break;
+      phys_col[n_phys] = -1;
+      fresh |= 1u << n_phys;
+      ++n_phys;
+    }
+    occ_last[s] = last[v];
+    phys[v] = s;
+  }
+  for (int v = 0; v < nv; ++v)
+    if (phys[v] < 0) {
+      err->set("the plan needs more than 8 values per row (input and computed columns), even with computed columns taking the slots of inputs they outlive: not supported");
+      return DBX_ERR_UNSUPPORTED;
+    }
+  // rewrite every slot reference
+  for (int i = 0; i < pl->n_nodes; ++i) {
+    PredNodeDev& n = pl->nodes[i];
+    if (n.kind == DBX_PRED_CMP) { n.l_slot = phys[n.l_slot]; if (n.r_slot >= 0) n.r_slot = phys[n.r_slot]; }
+    else if (n.kind == DBX_PRED_BOOLCOL) n.value = phys[n.value];
+  }
+  if (pl->grouped) {
+    for (int j = 0; j < pl->n_key_parts; ++j) pl->key_parts[j].slot = phys[pl->key_parts[j].slot];
+    pl->key_slot = phys[pl->key_slot];
+  }
+  for (int u = 0; u < pl->n_updates; ++u) pl->upd[u].slot = pl->upd[u].op == UPD_INC ? 0 : phys[pl->upd[u].slot];
+  pl->n_cnodes = 0;
+  pl->comp_nullable = false;
+  pl->can_raise = false;
+  for (int k = 0; k < n_ord; ++k) {
+    const int c = order[k];
+    if (pl->n_cnodes + pl->comp_n_nodes[c] > kMaxCompNodes) { err->set("computed columns: more than 32 expression nodes evaluated per row"); return DBX_ERR_UNSUPPORTED; }
+    int v = 0;
+    while (pl->slot_col[v] != pl->n_cols + c) ++v;
+    CompDev& cd = pl->comp[k];
+    memset(&cd, 0, sizeof(cd));
+    cd.first = pl->n_cnodes; cd.n_nodes = pl->comp_n_nodes[c]; cd.slot = phys[v];
+    for (int i = 0; i < pl->comp_n_nodes[c]; ++i) {
+      NodeDev nd = pl->comp_nodes[c][i];
+      if (nd.kind == DBX_EXPR_COLUMN) nd.col = phys[pl->slot_of(nd.col, err)];
+      pl->cnodes[pl->n_cnodes++] = nd;
+    }
+    pl->comp_nullable |= pl->col_nullable[pl->n_cols + c];
+    pl->can_raise |= pl->comp_raises[c];
+  }
+  pl->n_comp_ev = n_ord;
+  pl->comp_pred = n_pred;
+  pl->fresh_slots = fresh;
+  pl->n_slots = n_phys;
+  for (int s = 0; s < n_phys; ++s) pl->slot_col[s] = phys_col[s];
+  return DBX_OK;
+}
+
+int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols, const dbx_expr* comp, int32_t n_comp, AggPlan* pl,
+                   ErrorSink* err) {
   if (n_cols < 0 || n_cols > 64) { err->set("too many input columns"); return DBX_ERR_INVALID; }
   pl->params = *p;
   pl->n_cols = n_cols;
@@ -265,6 +433,8 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
     pl->col_dtype[i] = types[i] & 0xFF;
     pl->col_nullable[i] = (types[i] & DBX_NULLABLE) != 0;
   }
+  DBX_TRY(add_computed(pl, comp, n_comp, err));
+  n_cols += pl->n_comp;  // below, a column index may name a computed column
   if (p->n_aggs < 0 || p->n_aggs > DBX_MAX_AGGS) { err->set("bad aggregate count"); return DBX_ERR_INVALID; }
   if (p->n_group_cols < 0 || p->n_group_cols > DBX_MAX_GROUP_COLS) { err->set("bad group column count"); return DBX_ERR_INVALID; }
   DBX_TRY(lower_predicate(pl, p->filter, err));
@@ -319,8 +489,8 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
   memset(&pl->kinds, 0, sizeof(pl->kinds));
   pl->add_word(0, UPD_ADD_INT);
   pl->upd[pl->n_updates++] = UpdateDev{UPD_INC, 0, 0, 0, 0, 0};
-  int cnt_word_of_col[64], acc_word_of_col[64];
-  for (int i = 0; i < 64; ++i) cnt_word_of_col[i] = acc_word_of_col[i] = -1;
+  int cnt_word_of_col[kMaxCols], acc_word_of_col[kMaxCols];
+  for (int i = 0; i < kMaxCols; ++i) cnt_word_of_col[i] = acc_word_of_col[i] = -1;
 
   for (int a = 0; a < p->n_aggs; ++a) {
     const dbx_agg_desc& ad = p->aggs[a];
@@ -375,9 +545,10 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
     }
   }
   if (pl->n_slots == 0) {  // e.g. count(*) without filter: still need a row source
-    if (n_cols == 0) { err->set("operator needs at least one input column"); return DBX_ERR_INVALID; }
+    if (pl->n_cols == 0) { err->set("operator needs at least one input column"); return DBX_ERR_INVALID; }
     pl->slot_of(0, err);
   }
+  if (pl->n_comp) DBX_TRY(allocate_slots(pl, err));
   // Pair up additive words of the same class (integer adds incl. counters, or f64 adds), in
   // plan order: each pair costs one L2 reduction per row instead of two (the table phase is
   // bound by L2 atomic operations per row, not by bytes).
@@ -573,11 +744,15 @@ class AggPartialOp : public Op {
     }
   }
 
-  int32_t init(const dbx_agg_params* p, const int32_t* types, int32_t n, int dev) {
+  int32_t init(const dbx_agg_params* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int dev) {
     DBX_TRY(base_init(dev));
-    DBX_TRY(build_plan(p, types, n, &plan, &err));
+    DBX_TRY(build_plan(p, types, n, comp, n_comp, &plan, &err));
     DBX_TRY(stager.init(dev, stream, &err));
     DBX_CUDA_TRY(err, host_counters.ensure(64));
+    if (plan.can_raise) {
+      DBX_CUDA_TRY(err, expr_err.ensure(8));
+      DBX_CUDA_TRY(err, cudaMemsetAsync(expr_err.p, 0xFF, 8, stream));
+    }
     int64_t cap;
     if (!plan.grouped) cap = 4;
     else if (p->expected_groups > 0) cap = next_pow2(std::max<int64_t>(2 * p->expected_groups, 1024));
@@ -591,6 +766,9 @@ class AggPartialOp : public Op {
   std::string variant_text;
   const char* kernel_variant() override {
     variant_text = jit_status;
+    if (plan.n_comp_ev)  // which kernels evaluated the computed columns (tests assert the path they target)
+      variant_text += "; computed columns: straight-line launches " + std::to_string(comp_fast_launches) + ", generic launches " +
+                      std::to_string(comp_generic_launches) + ", rows absorbed by the hot-group cache " + std::to_string(hot_absorbed_seen);
     if (partitioned_chunks || partition_fallbacks)
       variant_text += "; two-pass (partitioned by table slice) chunks: " + std::to_string(partitioned_chunks) + " (pass 2 in shared memory: " +
                       std::to_string(slice_chunks) + ", in L2 regions: " + std::to_string(partitioned_chunks - slice_chunks) +
@@ -613,6 +791,11 @@ class AggPartialOp : public Op {
     memcpy(sp.upd, plan.upd, sizeof(UpdateDev) * plan.n_updates);
     for (int u = 0; u < plan.n_updates; ++u) sp.upd[u].ridx = plan.upd[u].word;  // no pairs: entry index == word index
     memcpy(sp.key_parts, plan.key_parts, sizeof(plan.key_parts));
+    if (plan.n_comp_ev) {
+      sp.n_comp = plan.n_comp_ev; sp.comp_pred = plan.comp_pred; sp.fresh_slots = plan.fresh_slots; sp.raises = plan.can_raise ? 1 : 0;
+      memcpy(sp.comp, plan.comp, sizeof(plan.comp));
+      memcpy(sp.cnodes, plan.cnodes, sizeof(NodeDev) * plan.n_cnodes);
+    }
     std::string why;
     if (!agg_jit_get(agg_jit_plan_text(sp), plan.n_slots, &jit, &why)) { jit = AggJitKernels(); jit_status = "precompiled kernels (" + why + ")"; return; }
     // the row stages of 5+ slots exceed the 48 KB default: opt the specialised kernels in on this device
@@ -707,6 +890,7 @@ class AggPartialOp : public Op {
     rows_since_read = 0;
     pulled = false;
     rows_in = 0;
+    if (plan.can_raise) DBX_CUDA_TRY(err, cudaMemsetAsync(expr_err.p, 0xFF, 8, stream));
     return DBX_OK;
   }
 
@@ -769,8 +953,14 @@ class AggPartialOp : public Op {
     DBX_CUDA_TRY(err, cudaGetLastError());
     return DBX_OK;
   }
+  int64_t comp_fast_launches = 0, comp_generic_launches = 0;
   template <int NS, bool FAST, bool INDIRECT>
   int32_t launch_one(const AggKernelParams& kp) {
+    // computed columns: the kernels that evaluate them (the ring and bulk variants do not: DESIGN §1, "Computed columns")
+    if (kp.n_comp > 0) {
+      ++(FAST ? comp_fast_launches : comp_generic_launches);
+      return launch_kernel<NS, FAST, INDIRECT, false, 4, true>(kp);
+    }
     // the TMA bulk-reduction variants exist for the straight-line kernel only; everywhere else
     // paired words are updated with plain REDs
     if (FAST && !INDIRECT && kp.n_pairs > 0 && plan.use_ring && ring_ok) return launch_ring<NS>(kp);
@@ -779,14 +969,14 @@ class AggPartialOp : public Op {
     // less latency)
     return launch_kernel<NS, FAST, INDIRECT, false, 4>(kp);
   }
-  template <int NS, bool FAST, bool INDIRECT, bool BULK, int MINB>
+  template <int NS, bool FAST, bool INDIRECT, bool BULK, int MINB, bool EXPR = false>
   int32_t launch_kernel(const AggKernelParams& kp) {
     static std::atomic<bool> attr_set[64];
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
     const size_t smem_rows = (sizeof(StageWarp<NS>) * kWarpsPerBlock + 15) & ~(size_t)15;
     const size_t smem_bulk = (size_t)kWarpsPerBlock * kBulkGen * kMaxPairs * 32 * 16;
     const size_t smem = smem_rows + (BULK ? smem_bulk : kHotBytes);  // the hot-group cache sits where the bulk staging would
-    auto kern = filter_group_agg_kernel<NS, FAST, INDIRECT, BULK, MINB>;
+    auto kern = filter_group_agg_kernel<NS, FAST, INDIRECT, BULK, MINB, EXPR>;
     if (!attr_set[device]) {
       DBX_CUDA_TRY(err, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       attr_set[device] = true;
@@ -808,31 +998,35 @@ class AggPartialOp : public Op {
     DBX_CUDA_TRY(err, cudaGetLastError());
     return DBX_OK;
   }
-  template <int NS, bool INDIRECT>
+  template <int NS, bool INDIRECT, bool EXPR>
   int32_t launch_wide(const AggKernelParams& kp) {
     static std::atomic<bool> attr_set[64];
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
     const size_t smem = (sizeof(StageWarp<NS>) * kWarpsPerBlock + 15) & ~(size_t)15;
     if (!attr_set[device]) {
-      DBX_CUDA_TRY(err, cudaFuncSetAttribute(filter_group_agg_wide_kernel<NS, INDIRECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      DBX_CUDA_TRY(err, cudaFuncSetAttribute(filter_group_agg_wide_kernel<NS, INDIRECT, EXPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       attr_set[device] = true;
     }
-    filter_group_agg_wide_kernel<NS, INDIRECT><<<grid_for_rows(kp.n_rows), kBlock, smem, stream>>>(kp);
+    filter_group_agg_wide_kernel<NS, INDIRECT, EXPR><<<grid_for_rows(kp.n_rows), kBlock, smem, stream>>>(kp);
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
     return DBX_OK;
   }
   template <bool INDIRECT>
   int32_t launch_wide_ns(const AggKernelParams& kp) {
+    return kp.n_comp > 0 ? launch_wide_slots<INDIRECT, true>(kp) : launch_wide_slots<INDIRECT, false>(kp);
+  }
+  template <bool INDIRECT, bool EXPR>
+  int32_t launch_wide_slots(const AggKernelParams& kp) {
     switch (plan.n_slots) {
-      case 1: return launch_wide<1, INDIRECT>(kp);
-      case 2: return launch_wide<2, INDIRECT>(kp);
-      case 3: return launch_wide<3, INDIRECT>(kp);
-      case 4: return launch_wide<4, INDIRECT>(kp);
-      case 5: return launch_wide<5, INDIRECT>(kp);
-      case 6: return launch_wide<6, INDIRECT>(kp);
-      case 7: return launch_wide<7, INDIRECT>(kp);
-      default: return launch_wide<8, INDIRECT>(kp);
+      case 1: return launch_wide<1, INDIRECT, EXPR>(kp);
+      case 2: return launch_wide<2, INDIRECT, EXPR>(kp);
+      case 3: return launch_wide<3, INDIRECT, EXPR>(kp);
+      case 4: return launch_wide<4, INDIRECT, EXPR>(kp);
+      case 5: return launch_wide<5, INDIRECT, EXPR>(kp);
+      case 6: return launch_wide<6, INDIRECT, EXPR>(kp);
+      case 7: return launch_wide<7, INDIRECT, EXPR>(kp);
+      default: return launch_wide<8, INDIRECT, EXPR>(kp);
     }
   }
   template <bool FAST, bool INDIRECT>
@@ -854,7 +1048,9 @@ class AggPartialOp : public Op {
     if (getenv("DBX_AGG_NO_FAST")) return false;
     if (kp.n_nodes > 1) return false;
     if (kp.n_nodes == 1 && (kp.nodes[0].kind != DBX_PRED_CMP || kp.nodes[0].r_slot >= 0)) return false;
+    if (kp.n_comp > 0 && plan.comp_nullable) return false;  // the straight-line kernel stages no validity
     for (int s = 0; s < kp.n_slots; ++s) {
+      if (kp.n_comp > 0 && ((kp.fresh_slots >> s) & 1)) continue;
       const DevCol& c = kp.cols[s];
       if (c.is_const || c.validity) return false;
       if (c.dtype != DBX_I64 && c.dtype != DBX_U64 && c.dtype != DBX_F64) return false;
@@ -879,18 +1075,23 @@ class AggPartialOp : public Op {
     }
     return DBX_OK;
   }
+  template <bool EXPR>
+  void launch_single_slots(const AggKernelParams& kp, int grid) {
+    switch (plan.n_slots) {
+      case 1: filter_single_agg_kernel<1, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      case 2: filter_single_agg_kernel<2, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      case 3: filter_single_agg_kernel<3, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      case 4: filter_single_agg_kernel<4, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      case 5: filter_single_agg_kernel<5, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      case 6: filter_single_agg_kernel<6, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      case 7: filter_single_agg_kernel<7, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+      default: filter_single_agg_kernel<8, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
+    }
+  }
   int32_t launch_single(const AggKernelParams& kp) {
     int grid = std::min(grid_for_rows(kp.n_rows), kNumSMs * 4);
-    switch (plan.n_slots) {
-      case 1: filter_single_agg_kernel<1><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 2: filter_single_agg_kernel<2><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 3: filter_single_agg_kernel<3><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 4: filter_single_agg_kernel<4><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 5: filter_single_agg_kernel<5><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 6: filter_single_agg_kernel<6><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 7: filter_single_agg_kernel<7><<<grid, kBlock, 0, stream>>>(kp); break;
-      default: filter_single_agg_kernel<8><<<grid, kBlock, 0, stream>>>(kp); break;
-    }
+    if (kp.n_comp > 0) launch_single_slots<true>(kp, grid);
+    else launch_single_slots<false>(kp, grid);
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
     return DBX_OK;
@@ -937,6 +1138,24 @@ class AggPartialOp : public Op {
     }
     kp->ring_nsv = 0;
     for (int s = 0; s < kMaxSlots; ++s) kp->ring_sidx[s] = (s < plan.n_slots && need[s]) ? (int8_t)kp->ring_nsv++ : (int8_t)-1;
+    // computed columns, except over pass 1's buffers (they hold the computed values already)
+    if (plan.n_comp_ev && !no_filter_) {
+      kp->n_comp = plan.n_comp_ev;
+      kp->comp_pred = plan.comp_pred;
+      kp->fresh_slots = plan.fresh_slots;
+      memcpy(kp->comp, plan.comp, sizeof(plan.comp));
+      memcpy(kp->cnodes, plan.cnodes, sizeof(NodeDev) * plan.n_cnodes);
+      kp->expr_row0 = expr_base + row0;
+      kp->expr_err = plan.can_raise ? (unsigned long long*)expr_err.p : nullptr;
+    }
+  }
+  // the DevCol of a slot that holds a computed value only: a constant, so the loads touch no memory
+  static DevCol fresh_col() {
+    DevCol c;
+    memset(&c, 0, sizeof(c));
+    c.dtype = DBX_U64;
+    c.is_const = 1;
+    return c;
   }
 
   int32_t push(const dbx_block* b) override {
@@ -959,8 +1178,11 @@ class AggPartialOp : public Op {
     // kernel runs once per ~4 Mi rows instead of once per block.
     if (batchable(b)) {
       if (batch_open && batch_rows + n > kBatchCapRows) DBX_TRY(flush_batch());
-      if (!batch_open) { DBX_TRY(stager.begin()); batch_open = true; batch_rows = 0; }
-      for (int s = 0; s < plan.n_slots; ++s) DBX_TRY(stager.stage_at(b->cols[plan.slot_col[s]], s, batch_rows, kBatchCapRows, &batch_cols[s]));
+      if (!batch_open) { DBX_TRY(stager.begin()); batch_open = true; batch_rows = 0; batch_row0 = rows_in; }
+      for (int s = 0; s < plan.n_slots; ++s) {
+        if (plan.slot_col[s] < 0) { batch_cols[s] = fresh_col(); continue; }
+        DBX_TRY(stager.stage_at(b->cols[plan.slot_col[s]], s, batch_rows, kBatchCapRows, &batch_cols[s]));
+      }
       batch_rows += n;
       rows_in += n;
       return DBX_OK;
@@ -968,7 +1190,11 @@ class AggPartialOp : public Op {
     DBX_TRY(flush_batch());
     DevCol cols[kMaxSlots];
     DBX_TRY(stager.begin());
-    for (int s = 0; s < plan.n_slots; ++s) DBX_TRY(stager.stage(b->cols[plan.slot_col[s]], s, &cols[s]));
+    for (int s = 0; s < plan.n_slots; ++s) {
+      if (plan.slot_col[s] < 0) { cols[s] = fresh_col(); continue; }
+      DBX_TRY(stager.stage(b->cols[plan.slot_col[s]], s, &cols[s]));
+    }
+    expr_base = rows_in;
     rows_in += n;
     DBX_TRY(process_rows(cols, n));
     DBX_TRY(stager.end());
@@ -980,10 +1206,15 @@ class AggPartialOp : public Op {
   static constexpr int64_t kBatchMaxBlockRows = 1 << 20;
   bool batch_open = false;
   int64_t batch_rows = 0;
+  int64_t batch_row0 = 0;  // number of the batch's first row since create / reset
+  int64_t expr_base = 0;   // number of the first row of the rows process_rows works on
+  DevBuf expr_err;         // plans that can raise: min over failing rows of (row << 8 | code), ~0: none
+  PinnedBuf expr_err_host;
   DevCol batch_cols[kMaxSlots];
   bool batchable(const dbx_block* b) const {
     if (no_batching || b->num_rows > kBatchMaxBlockRows) return false;
     for (int s = 0; s < plan.n_slots; ++s) {
+      if (plan.slot_col[s] < 0) continue;
       const dbx_column& c = b->cols[plan.slot_col[s]];
       if (c.mem != DBX_MEM_HOST || c.is_const || c.validity || c.dtype == DBX_BOOL) return false;
     }
@@ -999,6 +1230,7 @@ class AggPartialOp : public Op {
     if (!batch_open) return DBX_OK;
     batch_open = false;
     DBX_TRY(stager.join_aux());
+    expr_base = batch_row0;
     if (batch_rows > 0) DBX_TRY(process_rows(batch_cols, batch_rows));
     batch_rows = 0;
     DBX_TRY(stager.end());
@@ -1022,8 +1254,9 @@ class AggPartialOp : public Op {
     if ((int64_t)table.bytes() <= part_threshold || m < (1 << 16)) return false;
     // every partition pass pulls its table region into L2 again: worth it only when the rows outweigh the table
     if (m * 8 * plan.n_slots < 4 * (int64_t)table.bytes() && !getenv("DBX_AGG_PARTITION_ALWAYS")) return false;
+    if (plan.comp_nullable) return false;  // the partitions carry value images only
     for (int s = 0; s < plan.n_slots; ++s)
-      if (cols[s].is_const || cols[s].validity) return false;  // the partitions carry value images only
+      if (plan.slot_col[s] >= 0 && (cols[s].is_const || cols[s].validity)) return false;
     return true;
   }
   bool region_window_on = false;
@@ -1056,7 +1289,6 @@ class AggPartialOp : public Op {
   int64_t part_jit_launches = 0, slice_jit_launches = 0;
   template <int NS>
   int32_t launch_partition(const AggKernelParams& kp, const PartitionOut& po) {
-    static std::atomic<int> per_sm[64];  // resident CTAs per SM, 0: not asked yet
     const size_t smem = partition_smem_bytes<NS>();
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
     if (jit.two_pass_ok() && !jit_part_per_sm) {  // the occupancy of the kernel that will run
@@ -1072,15 +1304,22 @@ class AggPartialOp : public Op {
       if (ce == cudaSuccess) { ++part_jit_launches; return DBX_OK; }
       drop_two_pass_jit("launch", ce);
     }
+    if (kp.n_comp > 0) return launch_partition_kernel<NS, true>(kp, po);
+    return launch_partition_kernel<NS, false>(kp, po);
+  }
+  template <int NS, bool EXPR>
+  int32_t launch_partition_kernel(const AggKernelParams& kp, const PartitionOut& po) {
+    static std::atomic<int> per_sm[64];  // resident CTAs per SM, 0: not asked yet
+    const size_t smem = partition_smem_bytes<NS>();
     if (!per_sm[device]) {
-      cudaFuncSetAttribute(filter_partition_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaFuncSetAttribute(filter_partition_kernel<NS, EXPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       int n = 0;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, filter_partition_kernel<NS>, kBlock, smem);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, filter_partition_kernel<NS, EXPR>, kBlock, smem);
       per_sm[device] = std::max(1, n);
     }
     // one resident wave: a CTA copies its survivors out only every few tiles, more CTAs would only add partial batches
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * per_sm[device]));
-    filter_partition_kernel<NS><<<grid, kBlock, smem, stream>>>(kp, po);
+    filter_partition_kernel<NS, EXPR><<<grid, kBlock, smem, stream>>>(kp, po);
     return DBX_OK;
   }
   template <int NS>
@@ -1307,7 +1546,28 @@ class AggPartialOp : public Op {
     return DBX_OK;
   }
 
-  int32_t finish() override { return flush_batch(); }
+  // Plans whose computed columns can raise read the error word here (the one synchronisation they add);
+  // a failure poisons the operator until reset, so no state built from the failed input leaves it.
+  int32_t finish() override {
+    DBX_TRY(flush_batch());
+    return check_expr_error();
+  }
+  // Every hand-off of the partial's state (finish, merge into a final, partition / serialize, exchange)
+  // runs this after flushing, so state built from rows that failed to evaluate never leaves the operator.
+  int32_t check_expr_error() {
+    if (poisoned) { err.set(poison_msg); return DBX_ERR_STATE; }
+    if (!plan.can_raise) return DBX_OK;
+    DBX_CUDA_TRY(err, expr_err_host.ensure(8));
+    DBX_CUDA_TRY(err, cudaMemcpyAsync(expr_err_host.p, expr_err.p, 8, cudaMemcpyDeviceToHost, stream));
+    DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
+    const unsigned long long w = *(const unsigned long long*)expr_err_host.p;
+    if (w == ~0ULL) return DBX_OK;
+    const int code = (int)(w & 0xFF);
+    const int64_t row = (int64_t)(w >> 8);
+    const char* msg = code == ERR_DIV_ZERO ? "Division by zero" : code == ERR_DIVIDED_BY_ZERO ? "divided by zero" : "number overflowed";
+    poison(std::string(msg) + " while evaluating a computed column (first failing row " + std::to_string(row) + ")");
+    return DBX_ERR_BAD_ARGUMENTS;
+  }
 
   // The partial emits one metadata-only block (AggregateMeta::AggregatePayload): the payload
   // stays in HBM and is referenced through block.meta.
@@ -1352,9 +1612,9 @@ class AggFinalOp : public Op {
   bool fin_timed = false;
   ~AggFinalOp() override { if (ev_fin_end) cudaEventDestroy(ev_fin_end); }
 
-  int32_t init(const dbx_agg_params* p, const int32_t* types, int32_t n, int dev) {
+  int32_t init(const dbx_agg_params* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int dev) {
     DBX_TRY(base_init(dev));
-    DBX_TRY(build_plan(p, types, n, &plan, &err));
+    DBX_TRY(build_plan(p, types, n, comp, n_comp, &plan, &err));
     DBX_CUDA_TRY(err, host_counters.ensure(64));
     DBX_CUDA_TRY(err, cudaEventCreate(&ev_fin_end));
     return DBX_OK;
@@ -1416,6 +1676,7 @@ class AggFinalOp : public Op {
     }
     {
       int32_t st = part->flush_batch();
+      if (st == DBX_OK) st = part->check_expr_error();
       if (st == DBX_OK) st = part->ensure_table();
       if (st != DBX_OK) { err.set(part->err.msg); return st; }
     }
@@ -1679,12 +1940,12 @@ class FilterOp : public Op {
   size_t out_head = 0;
   int64_t rows_in = 0, rows_out = 0;
 
-  int32_t init(const dbx_predicate* pred, const int32_t* types, int32_t n, int dev) {
+  int32_t init(const dbx_predicate* pred, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int dev) {
     DBX_TRY(base_init(dev));
     dbx_agg_params ap;
     memset(&ap, 0, sizeof(ap));
     ap.filter = *pred;
-    DBX_TRY(build_plan(&ap, types, n, &plan, &err));
+    DBX_TRY(build_plan(&ap, types, n, comp, n_comp, &plan, &err));
     for (int i = 0; i < n; ++i)
       if (plan.col_dtype[i] != DBX_BOOL && dtype_size(plan.col_dtype[i]) == 0) { err.set("filter: unsupported column type (numeric and boolean columns only)"); return DBX_ERR_UNSUPPORTED; }
     DBX_TRY(stager.init(dev, stream, &err));
@@ -1696,7 +1957,8 @@ class FilterOp : public Op {
 
   template <int NS>
   void launch_select(const AggKernelParams& kp, int grid) {
-    filter_select_kernel<NS><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
+    if (kp.n_comp > 0) filter_select_kernel<NS, true><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
+    else filter_select_kernel<NS><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
   }
 
   int32_t push(const dbx_block* b) override {
@@ -1723,7 +1985,11 @@ class FilterOp : public Op {
       DBX_TRY(stager.begin());
       int col_slot[64];
       for (int c = 0; c < plan.n_cols; ++c) col_slot[c] = -1;
-      for (int s = 0; s < plan.n_slots; ++s) { DBX_TRY(stager.stage(b->cols[plan.slot_col[s]], s, &pcols[s])); col_slot[plan.slot_col[s]] = s; }
+      for (int s = 0; s < plan.n_slots; ++s) {
+        if (plan.slot_col[s] < 0) { memset(&pcols[s], 0, sizeof(DevCol)); pcols[s].dtype = DBX_U64; pcols[s].is_const = 1; continue; }
+        DBX_TRY(stager.stage(b->cols[plan.slot_col[s]], s, &pcols[s]));
+        col_slot[plan.slot_col[s]] = s;
+      }
       for (int c = 0; c < plan.n_cols; ++c) {
         if (col_slot[c] >= 0) ccols[c] = pcols[col_slot[c]];
         else DBX_TRY(stager.stage(b->cols[c], plan.n_slots + c, &ccols[c]));
@@ -1736,6 +2002,11 @@ class FilterOp : public Op {
       for (int s = 0; s < plan.n_slots; ++s) kp.cols[s] = pcols[s];
       memcpy(kp.nodes, plan.nodes, sizeof(PredNodeDev) * plan.n_nodes);
       kp.n_rows = n; kp.n_slots = plan.n_slots; kp.n_nodes = plan.n_nodes; kp.key_slot = -1;
+      if (plan.n_comp_ev) {  // computed predicate operands (they cannot raise: allocate_slots refuses those)
+        kp.n_comp = plan.n_comp_ev; kp.comp_pred = plan.comp_pred; kp.fresh_slots = plan.fresh_slots;
+        memcpy(kp.comp, plan.comp, sizeof(plan.comp));
+        memcpy(kp.cnodes, plan.cnodes, sizeof(NodeDev) * plan.n_cnodes);
+      }
       const int grid = grid_for_rows(n);
       DBX_TRY(timing_begin());
       switch (plan.n_slots) {
@@ -1837,22 +2108,24 @@ class FilterOp : public Op {
   }
 };
 
-Op* make_filter_op(const dbx_predicate* p, const int32_t* types, int32_t n, int device, int32_t* st) {
+Op* make_filter_op(const dbx_predicate* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device, int32_t* st) {
   auto* op = new FilterOp();
-  *st = op->init(p, types, n, device);
+  *st = op->init(p, types, n, comp, n_comp, device);
   if (*st != DBX_OK) { g_create_error.set(op->err.msg); delete op; return nullptr; }
   return op;
 }
 
-Op* make_agg_partial_op(const dbx_agg_params* p, const int32_t* types, int32_t n, int device, int32_t* st) {
+Op* make_agg_partial_op(const dbx_agg_params* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device,
+                        int32_t* st) {
   auto* op = new AggPartialOp();
-  *st = op->init(p, types, n, device);
+  *st = op->init(p, types, n, comp, n_comp, device);
   if (*st != DBX_OK) { g_create_error.set(op->err.msg); delete op; return nullptr; }
   return op;
 }
-Op* make_agg_final_op(const dbx_agg_params* p, const int32_t* types, int32_t n, int device, int32_t* st) {
+Op* make_agg_final_op(const dbx_agg_params* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device,
+                      int32_t* st) {
   auto* op = new AggFinalOp();
-  *st = op->init(p, types, n, device);
+  *st = op->init(p, types, n, comp, n_comp, device);
   if (*st != DBX_OK) { g_create_error.set(op->err.msg); delete op; return nullptr; }
   return op;
 }
@@ -1881,6 +2154,7 @@ int32_t dbx_agg_partial_partition(dbx_op* partial_op, int32_t n_parts, void** de
   if (p->plan.key_words != 1) { p->err.set("128-bit packed group keys: the row exchange / serialisation formats carry 64-bit keys only (single-GPU partial -> final hand-off works)"); return DBX_ERR_UNSUPPORTED; }
   DBX_CUDA_TRY(p->err, cudaSetDevice(p->device));
   DBX_TRY(p->flush_batch());
+  DBX_TRY(p->check_expr_error());
   DevBuf counts;
   DBX_CUDA_TRY(p->err, counts.ensure((size_t)n_parts * 8));
   DBX_CUDA_TRY(p->err, cudaMemsetAsync(counts.p, 0, (size_t)n_parts * 8, p->stream));
@@ -2215,7 +2489,7 @@ int32_t dbx_agg_exchange_scatter(dbx_agg_exchange* x, dbx_op* partial_op) {
   if (!x->connected) { x->err.set("exchange: scatter before connect"); return DBX_ERR_STATE; }
   AggPartialOp* p = static_cast<AggPartialOp*>(reinterpret_cast<Op*>(partial_op));
   DBX_CUDA_TRY(x->err, cudaSetDevice(x->device));
-  { int32_t st = p->flush_batch(); if (st == DBX_OK) st = p->ensure_table(); if (st != DBX_OK) { x->err.set(p->err.msg); return st; } }
+  { int32_t st = p->flush_batch(); if (st == DBX_OK) st = p->check_expr_error(); if (st == DBX_OK) st = p->ensure_table(); if (st != DBX_OK) { x->err.set(p->err.msg); return st; } }
   if (2 + p->plan.n_words != x->row_words) { x->err.set("exchange: operator state layout differs from the exchange's"); return DBX_ERR_INVALID; }
   x->epoch += 1;
   // region reuse: this rank's merge of the previous epoch must precede the scatter that lets peers move on

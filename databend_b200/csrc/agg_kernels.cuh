@@ -26,14 +26,20 @@ namespace dbx {
 // shape) defines DBX_JIT and a `__device__ constexpr StaticPlan jit_plan` before including this
 // header: every plan field then is a compile-time constant, the update / predicate loops unroll and
 // the per-row interpretation (op if-chains, slot selects, runtime-shift rotates) folds away.
+// Computed columns: the precompiled kernels take them through a template flag (EXPR), so that the
+// instantiations serving plans without them stay as they were; a specialised build knows from the plan.
 #ifdef DBX_JIT
 #define PLN(f) (jit_plan.f)
 #define PLN_TABLE(f) (jit_plan.f)
 #define PLN_UNROLL _Pragma("unroll")
+#define PLN_COMP(EXPR) (jit_plan.n_comp > 0)
+#define PLN_RAISES (jit_plan.raises != 0)
 #else
 #define PLN(f) (p.f)
 #define PLN_TABLE(f) (p.table.f)
 #define PLN_UNROLL
+#define PLN_COMP(EXPR) (EXPR)
+#define PLN_RAISES (p.expr_err != nullptr)
 #endif
 
 constexpr int kBlock = 256;       // threads per CTA
@@ -159,6 +165,98 @@ __device__ __forceinline__ uint32_t pick_mask(const uint32_t (&m)[NS], int slot)
   for (int s = 1; s < NS; ++s)
     if (slot == s) r = m[s];
   return r;
+}
+
+// ---------------------------------------------------------------- computed columns
+// One computed column's postfix program on one row: a value stack held in registers (push / pop shift
+// them), COLUMN nodes read the row's slot values v[] / validity bits.  Returns the value (0 when NULL).
+template <typename V>
+__device__ __forceinline__ uint64_t comp_row(const CompDev& cd, const NodeDev* cnodes, const V& v, uint32_t valid, bool& ok, int& err) {
+  uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0;
+  bool n0 = false, n1 = false, n2 = false, n3 = false, n4 = false, n5 = false, n6 = false, n7 = false;
+  PLN_UNROLL
+  for (int i = cd.first; i < cd.first + cd.n_nodes; ++i) {
+    const NodeDev nd = cnodes[i];
+    if (nd.kind == DBX_EXPR_COLUMN || nd.kind == DBX_EXPR_CONST) {
+      s7 = s6; s6 = s5; s5 = s4; s4 = s3; s3 = s2; s2 = s1; s1 = s0;
+      n7 = n6; n6 = n5; n5 = n4; n4 = n3; n3 = n2; n2 = n1; n1 = n0;
+      if (nd.kind == DBX_EXPR_COLUMN) { n0 = (valid >> nd.col) & 1; s0 = n0 ? v[nd.col] : 0; }
+      else { n0 = !nd.c_null; s0 = n0 ? nd.c_bits : 0; }
+    } else if (nd.kind == DBX_EXPR_CAST) {
+      apply_cast(nd, s0, n0, err);
+    } else if (nd.func == DBX_FN_NOT || nd.func == DBX_FN_NEGATE || nd.func == DBX_FN_IS_NULL || nd.func == DBX_FN_IS_NOT_NULL) {
+      apply_unary(nd, s0, n0, err);
+    } else {
+      apply_binary(nd, s1, n1, s0, n0, err);  // s1 op s0 -> s1, then pop
+      s0 = s1; s1 = s2; s2 = s3; s3 = s4; s4 = s5; s5 = s6; s6 = s7;
+      n0 = n1; n1 = n2; n2 = n3; n3 = n4; n4 = n5; n5 = n6; n6 = n7;
+    }
+  }
+  ok = n0;
+  return n0 ? s0 : 0;
+}
+#ifndef DBX_JIT
+// The precompiled kernels share ONE out-of-line copy of the interpreter (inlined into every
+// instantiation it would multiply their code and build time); a specialised build inlines comp_row
+// with constexpr nodes, where it folds into straight-line code.  Under the 64-register bound of these
+// kernels the call costs spills (DESIGN §4: computed columns); the specialised build has none of them.
+struct SlotRow { uint64_t v[kMaxSlots]; };
+struct CompOut { uint64_t v; int32_t ok, err; };
+static __device__ __noinline__ CompOut comp_row_interp(const AggKernelParams& p, int c, const SlotRow row, uint32_t valid) {
+  bool o = false;
+  int e = 0;
+  CompOut r;
+  r.v = comp_row(p.comp[c], p.cnodes, row.v, valid, o, e);
+  r.ok = o;
+  r.err = e;
+  return r;
+}
+#endif
+
+// Evaluates computed columns [c0, c1) on the thread's rows (EvalScalar between the filter and the
+// aggregate, fused); the result replaces the value and validity of the column's slot.  A failing call is
+// recorded only on rows of `record` (rows the predicate kept), as the first failing row since the
+// operator's create / reset.
+template <int NS, bool INDIRECT>
+__device__ __forceinline__ void eval_computed(const AggKernelParams& p, int c0, int c1, RowVals (&vals)[NS], uint32_t (&vmask)[NS],
+                                              uint32_t record, int64_t r0) {
+  PLN_UNROLL
+  for (int c = c0; c < c1; ++c) {
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j) {
+      uint32_t valid = 0;
+#pragma unroll
+      for (int s = 0; s < NS; ++s) valid |= ((vmask[s] >> j) & 1u) << s;
+      bool ok = false;
+      int err = 0;
+#ifdef DBX_JIT
+      uint64_t v[NS];
+#pragma unroll
+      for (int s = 0; s < NS; ++s) v[s] = vals[s].v[j];
+      const CompDev cd = PLN(comp[c]);
+      const uint64_t out = comp_row(cd, jit_plan.cnodes, v, valid, ok, err);
+#else
+      SlotRow row;
+#pragma unroll
+      for (int s = 0; s < kMaxSlots; ++s) row.v[s] = s < NS ? vals[s].v[j] : 0;
+      const CompOut co = comp_row_interp(p, c, row, valid);
+      const uint64_t out = co.v;
+      ok = co.ok != 0;
+      err = co.err;
+      const CompDev cd = p.comp[c];
+#endif
+      if (PLN_RAISES && err && ((record >> j) & 1)) {
+        const int64_t row = p.expr_row0 + (INDIRECT ? (int64_t)p.row_index[r0 + j] : (int64_t)p.row_base + r0 + j);
+        atomicMin(p.expr_err, ((unsigned long long)row << 8) | (unsigned long long)err);
+      }
+#pragma unroll
+      for (int s = 0; s < NS; ++s)
+        if (s == cd.slot) {
+          vals[s].v[j] = out;
+          vmask[s] = (vmask[s] & ~(1u << j)) | ((ok ? 1u : 0u) << j);
+        }
+    }
+  }
 }
 
 // OrderedFloat compare (src/common/base/src/base/ordered_float.rs:147-201)
@@ -575,16 +673,17 @@ __device__ __forceinline__ void table_phase32(const AggKernelParams& p, const St
   __syncwarp();
 }
 
-template <int NS>
+template <int NS, bool EXPR = false>
 __device__ __forceinline__ void prefetch_tile(const AggKernelParams& p, int64_t tile, RowVals (&vals)[NS]) {
 #pragma unroll
   for (int s = 0; s < NS; ++s) {
+    if (PLN_COMP(EXPR) && ((PLN(fresh_slots) >> s) & 1)) continue;  // a computed column's own slot: nothing to load
     u64x4 q = ld_stream_256((const char*)p.cols[s].data + (tile * kTileRows + (int64_t)kRowsPerThread * threadIdx.x) * 8);
     vals[s].v[0] = q.x; vals[s].v[1] = q.y; vals[s].v[2] = q.z; vals[s].v[3] = q.w;
   }
 }
 
-template <int NS, bool FAST, bool INDIRECT, bool BULK, int KW = 1>
+template <int NS, bool FAST, bool INDIRECT, bool BULK, int KW = 1, bool EXPR = false>
 __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -618,7 +717,7 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
   for (int s = 0; s < NS; ++s) vmask[s] = 0xF;
 
   int64_t tile = blockIdx.x;
-  if (FAST && tile < n_tiles) prefetch_tile<NS>(p, tile, vals);
+  if (FAST && tile < n_tiles) prefetch_tile<NS, EXPR>(p, tile, vals);
   for (; tile < n_tiles; tile += gridDim.x) {
     __syncwarp();  // lanes enter every tile together (diverged lanes would serialise the warp)
     const int64_t tile_base = tile * kTileRows;
@@ -626,6 +725,7 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
     uint32_t sel;
     if (FAST) {
       sel = 0xF;
+      if (PLN_COMP(EXPR)) eval_computed<NS, INDIRECT>(p, 0, PLN(comp_pred), vals, vmask, 0, r0);
       if (PLN(n_nodes)) {
         const PredNodeDev nd = PLN(nodes[0]);
 #pragma unroll
@@ -639,8 +739,10 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
 #pragma unroll
       for (int j = 0; j < kRowsPerThread; ++j)
         if (r0 + j < p.n_rows) in_range |= 1u << j;
+      if (PLN_COMP(EXPR)) eval_computed<NS, INDIRECT>(p, 0, PLN(comp_pred), vals, vmask, 0, r0);
       sel = eval_predicate<NS>(p, vals, vmask, in_range);
     }
+    if (PLN_COMP(EXPR)) eval_computed<NS, INDIRECT>(p, PLN(comp_pred), PLN(n_comp), vals, vmask, sel, r0);
     if (PLN(debug_flags) & 2) sel = 0;
     // ballot compaction: append the surviving rows behind the carried-over ones
 #pragma unroll
@@ -662,7 +764,7 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
     }
     if (FAST) {  // prefetch the next tile: the loads fly while this warp works on the table
       const int64_t nt = tile + gridDim.x;
-      if (nt < n_tiles) prefetch_tile<NS>(p, nt, vals);
+      if (nt < n_tiles) prefetch_tile<NS, EXPR>(p, nt, vals);
     }
     __syncwarp();
     while (n_staged >= 32) {
@@ -706,14 +808,14 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
 }
 
 #ifndef DBX_JIT
-template <int NS, bool FAST, bool INDIRECT, bool BULK = false, int MINB = 4>
+template <int NS, bool FAST, bool INDIRECT, bool BULK = false, int MINB = 4, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock, MINB) filter_group_agg_kernel(const __grid_constant__ AggKernelParams p) {
-  filter_group_agg_body<NS, FAST, INDIRECT, BULK>(p);
+  filter_group_agg_body<NS, FAST, INDIRECT, BULK, 1, EXPR>(p);
 }
 // 128-bit packed group keys (two key words per slot): any column layout, direct or replayed rows
-template <int NS, bool INDIRECT>
+template <int NS, bool INDIRECT, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock, 4) filter_group_agg_wide_kernel(const __grid_constant__ AggKernelParams p) {
-  filter_group_agg_body<NS, false, INDIRECT, false, 2>(p);
+  filter_group_agg_body<NS, false, INDIRECT, false, 2, EXPR>(p);
 }
 #endif
 
@@ -795,7 +897,7 @@ __device__ __forceinline__ void block_exclusive_scan(const unsigned int* cnt, un
   __syncthreads();
 }
 
-template <int NS>
+template <int NS, bool EXPR = false>
 __device__ __forceinline__ void filter_partition_body(const AggKernelParams& p, const PartitionOut& po) {
   constexpr int R = partition_stash_rows<NS>();
   // dynamic shared memory: [NS][R] survivors in arrival order, [R] tags (partition << 16 | rank), [R] copy-out order
@@ -829,7 +931,10 @@ __device__ __forceinline__ void filter_partition_body(const AggKernelParams& p, 
 #pragma unroll
     for (int j = 0; j < kRowsPerThread; ++j)
       if (r0 + j < p.n_rows) in_range |= 1u << j;
+    // computed values are stashed with the inputs: pass 2 reads them and evaluates nothing
+    if (PLN_COMP(EXPR)) eval_computed<NS, false>(p, 0, PLN(comp_pred), vals, vmask, 0, r0);
     const uint32_t sel = eval_predicate<NS>(p, vals, vmask, in_range);
+    if (PLN_COMP(EXPR)) eval_computed<NS, false>(p, PLN(comp_pred), PLN(n_comp), vals, vmask, sel, r0);
     uint32_t tg[kRowsPerThread], bal[kRowsPerThread];
     int warp_n = 0;
 #pragma unroll
@@ -1180,9 +1285,9 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
 
 #ifndef DBX_JIT  // everything below is compiled offline only
 // the precompiled passes (no NVRTC on the machine, a plan that could not be specialised, DBX_AGG_JIT=0)
-template <int NS>
+template <int NS, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ PartitionOut po) {
-  filter_partition_body<NS>(p, po);
+  filter_partition_body<NS, EXPR>(p, po);
 }
 template <int NS>
 __global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ SliceIn si) {
@@ -1367,7 +1472,7 @@ __device__ __forceinline__ void merge_word(int op, void* w, uint64_t v) {
   red_add_u64(w, v);
 }
 
-template <int NS>
+template <int NS, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock, 4) filter_single_agg_kernel(const __grid_constant__ AggKernelParams p) {
   const int64_t n_tiles = (p.n_rows + kTileRows - 1) / kTileRows;
   __shared__ uint64_t s_acc[kWarpsPerBlock][kMaxUpdates];
@@ -1396,7 +1501,9 @@ __global__ void __launch_bounds__(kBlock, 4) filter_single_agg_kernel(const __gr
 #pragma unroll
     for (int j = 0; j < kRowsPerThread; ++j)
       if (r0 + j < p.n_rows) in_range |= 1u << j;
+    if (EXPR) eval_computed<NS, false>(p, 0, p.comp_pred, vals, vmask, 0, r0);
     const uint32_t sel = eval_predicate<NS>(p, vals, vmask, in_range);
+    if (EXPR) eval_computed<NS, false>(p, p.comp_pred, p.n_comp, vals, vmask, sel, r0);
     for (int u = 0; u < p.n_updates; ++u) {
       const UpdateDev ud = p.upd[u];
       const uint32_t m = sel & (ud.op == UPD_INC ? 0xFu : pick_mask<NS>(vmask, ud.slot));
@@ -1442,7 +1549,7 @@ __global__ void __launch_bounds__(kBlock, 4) filter_single_agg_kernel(const __gr
 //   (scan of the tile counts)
 //   pass 2  filter_take_kernel: every thread knows its output position (tile offset + block scan of
 //           the popcounts) and copies its selected rows of every column — order preserved, no atomics.
-template <int NS>
+template <int NS, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock) filter_select_kernel(const __grid_constant__ AggKernelParams p, uint8_t* sel_nibbles,
                                                                uint32_t* tile_counts) {
   __shared__ uint32_t s_cnt[kWarpsPerBlock];
@@ -1460,6 +1567,7 @@ __global__ void __launch_bounds__(kBlock) filter_select_kernel(const __grid_cons
 #pragma unroll
     for (int j = 0; j < kRowsPerThread; ++j)
       if (r0 + j < p.n_rows) in_range |= 1u << j;
+    if (EXPR) eval_computed<NS, false>(p, 0, p.n_comp, vals, vmask, 0, r0);  // predicate inputs only: they cannot raise
     const uint32_t sel = eval_predicate<NS>(p, vals, vmask, in_range);
     sel_nibbles[tile * kBlock + threadIdx.x] = (uint8_t)sel;
     uint32_t c = __popc(sel);

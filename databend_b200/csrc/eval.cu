@@ -65,6 +65,34 @@ inline int type_modulo(int a, int b) {
 }
 inline int type_negate(int a) { return is_float_t(a) ? a : make_type(next_bits(bits_of_t(a)), true, false); }
 
+// The interpreter: an 8-deep value stack held in registers (push / pop shift the registers, so no
+// dynamically indexed local array), top of stack in s0.
+__global__ void __launch_bounds__(256) eval_kernel(const __grid_constant__ EvalParams p) {
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows; r += (int64_t)gridDim.x * blockDim.x) {
+    uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0;
+    bool n0 = false, n1 = false, n2 = false, n3 = false, n4 = false, n5 = false, n6 = false, n7 = false;
+    int err = 0;
+    for (int i = 0; i < p.n_nodes; ++i) {
+      const NodeDev& nd = p.nodes[i];
+      if (nd.kind == DBX_EXPR_COLUMN || nd.kind == DBX_EXPR_CONST) {
+        s7 = s6; s6 = s5; s5 = s4; s4 = s3; s3 = s2; s2 = s1; s1 = s0;
+        n7 = n6; n6 = n5; n5 = n4; n4 = n3; n3 = n2; n2 = n1; n1 = n0;
+        if (nd.kind == DBX_EXPR_COLUMN) load_column(p.cols[nd.col], r, nd.out, s0, n0);
+        else { s0 = nd.c_bits; n0 = !nd.c_null; }
+      } else if (nd.kind == DBX_EXPR_CAST) {
+        apply_cast(nd, s0, n0, err);
+      } else if (nd.func == DBX_FN_NOT || nd.func == DBX_FN_NEGATE || nd.func == DBX_FN_IS_NULL || nd.func == DBX_FN_IS_NOT_NULL) {
+        apply_unary(nd, s0, n0, err);
+      } else {
+        apply_binary(nd, s1, n1, s0, n0, err);  // s1 op s0 -> s1, then pop
+        s0 = s1; s1 = s2; s2 = s3; s3 = s4; s4 = s5; s5 = s6; s6 = s7;
+        n0 = n1; n1 = n2; n2 = n3; n3 = n4; n4 = n5; n5 = n6; n6 = n7;
+      }
+    }
+    store_result(p, r, s0, n0, err);
+  }
+}
+
 // Source of the straight-line kernel for a type-checked program: every node is a constexpr
 // NodeDev, every stack slot a named variable.
 std::string specialised_source(const EvalParams& p) {
@@ -97,38 +125,26 @@ std::string specialised_source(const EvalParams& p) {
 }
 
 }  // namespace
-}  // namespace dbx
 
-using namespace dbx;
-
-extern "C" int32_t dbx_eval_scalar(int32_t device, const dbx_expr* expr, const dbx_block* block, int32_t out_mem, dbx_block* out,
-                                   int32_t* out_dtype, int64_t* first_error_row) {
-  ErrorSink& err = g_create_error;
-  if (!expr || !block || !out || expr->n_nodes < 1 || expr->n_nodes > kMaxExprNodes || block->num_cols > 16) { err.set("dbx_eval_scalar: bad argument"); return DBX_ERR_INVALID; }
-  if (first_error_row) *first_error_row = -1;
-  int32_t ndev = 0;
-  DBX_TRY(dbx_device_count(&ndev));
-  if (device < 0 || device >= ndev) { err.set("dbx_eval_scalar: device index out of range"); return DBX_ERR_INVALID; }
-  DBX_CUDA_TRY(err, cudaSetDevice(device));
-  const int64_t n = block->num_rows;
-  // ---- type inference over the postfix program
-  EvalParams p;
-  memset(&p, 0, sizeof(p));
+int32_t infer_expr_types(const dbx_expr& expr, int n_cols, const int* col_dtype, const bool* col_nullable, NodeDev* nodes,
+                         int* out_dtype, bool* out_nullable, ErrorSink& err) {
+  if (expr.n_nodes < 1 || expr.n_nodes > kMaxExprNodes) { err.set("eval: bad node count"); return DBX_ERR_INVALID; }
   int tstack[kEvalStack];
   bool nstack[kEvalStack];  // nullable
   int sp = 0;
   auto numeric = [](int t) { return t != DBX_BOOL && t != DBX_VEC_F32 && dtype_size(t) > 0; };
-  for (int i = 0; i < expr->n_nodes; ++i) {
-    const dbx_expr_node& in = expr->nodes[i];
-    NodeDev& nd = p.nodes[i];
+  for (int i = 0; i < expr.n_nodes; ++i) {
+    const dbx_expr_node& in = expr.nodes[i];
+    NodeDev& nd = nodes[i];
+    memset(&nd, 0, sizeof(nd));
     nd.kind = in.kind; nd.func = in.func;
     if (in.kind == DBX_EXPR_COLUMN) {
-      if (in.col < 0 || in.col >= block->num_cols) { err.set("eval: column index outside the block"); return DBX_ERR_INVALID; }
-      const dbx_column& c = block->cols[in.col];
-      if (c.dtype == DBX_VEC_F32 || (c.dtype != DBX_BOOL && dtype_size(c.dtype) == 0)) { err.set("eval: only numeric and boolean columns"); return DBX_ERR_UNSUPPORTED; }
+      if (in.col < 0 || in.col >= n_cols) { err.set("eval: column index outside the block"); return DBX_ERR_INVALID; }
+      const int dt = col_dtype[in.col];
+      if (dt == DBX_VEC_F32 || (dt != DBX_BOOL && dtype_size(dt) == 0)) { err.set("eval: only numeric and boolean columns"); return DBX_ERR_UNSUPPORTED; }
       if (sp >= kEvalStack) { err.set("eval: expression too deep"); return DBX_ERR_UNSUPPORTED; }
-      nd.col = in.col; nd.out = c.dtype;
-      tstack[sp] = c.dtype; nstack[sp] = c.validity != nullptr || (c.is_const && c.konst.is_null); ++sp;
+      nd.col = in.col; nd.out = dt;
+      tstack[sp] = dt; nstack[sp] = col_nullable[in.col]; ++sp;
     } else if (in.kind == DBX_EXPR_CONST) {
       if (sp >= kEvalStack) { err.set("eval: expression too deep"); return DBX_ERR_UNSUPPORTED; }
       const int t = in.c.dtype;
@@ -182,8 +198,65 @@ extern "C" int32_t dbx_eval_scalar(int32_t device, const dbx_expr* expr, const d
     } else { err.set("eval: unknown node kind"); return DBX_ERR_INVALID; }
   }
   if (sp != 1) { err.set("eval: postfix program does not reduce to one value"); return DBX_ERR_INVALID; }
-  const int ot = tstack[0];
-  const bool o_nullable = nstack[0];
+  *out_dtype = tstack[0];
+  *out_nullable = nstack[0];
+  return DBX_OK;
+}
+
+namespace {
+// can `x as to` (checked: checked_cast) fail for some value x of type `from`?
+bool cast_can_overflow(int from, int to) {
+  if (to == DBX_BOOL || is_float_t(to) || from == DBX_BOOL) return false;
+  if (is_float_t(from)) return true;
+  const int fb = bits_of_t(from), tb = bits_of_t(to);
+  if (is_signed_t(from) == is_signed_t(to)) return fb > tb;
+  if (is_signed_t(from)) return true;  // negative values never fit an unsigned type
+  return fb >= tb;                     // unsigned into signed needs one more bit
+}
+}  // namespace
+
+bool expr_can_raise(const NodeDev* nodes, int n_nodes) {
+  for (int i = 0; i < n_nodes; ++i) {
+    const NodeDev& n = nodes[i];
+    if (n.kind == DBX_EXPR_CAST && !n.try_cast && cast_can_overflow(n.a_type, n.out)) return true;
+    if (n.kind != DBX_EXPR_CALL) continue;
+    if (n.func == DBX_FN_NEGATE && (n.a_type == DBX_I64 || n.a_type == DBX_U64)) return true;
+    if (n.func == DBX_FN_DIVIDE || n.func == DBX_FN_DIV || n.func == DBX_FN_MODULO) {
+      const NodeDev& d = nodes[i - 1];  // the divisor is the node right below the call when it is a constant
+      const bool const_divisor = d.kind == DBX_EXPR_CONST;
+      const bool zero = is_float_t(d.out) ? (d.c_bits << 1) == 0 : d.c_bits == 0;
+      if (!const_divisor || (!d.c_null && zero)) return true;
+    }
+  }
+  return false;
+}
+
+}  // namespace dbx
+
+using namespace dbx;
+
+extern "C" int32_t dbx_eval_scalar(int32_t device, const dbx_expr* expr, const dbx_block* block, int32_t out_mem, dbx_block* out,
+                                   int32_t* out_dtype, int64_t* first_error_row) {
+  ErrorSink& err = g_create_error;
+  if (!expr || !block || !out || expr->n_nodes < 1 || expr->n_nodes > kMaxExprNodes || block->num_cols > 16) { err.set("dbx_eval_scalar: bad argument"); return DBX_ERR_INVALID; }
+  if (first_error_row) *first_error_row = -1;
+  int32_t ndev = 0;
+  DBX_TRY(dbx_device_count(&ndev));
+  if (device < 0 || device >= ndev) { err.set("dbx_eval_scalar: device index out of range"); return DBX_ERR_INVALID; }
+  DBX_CUDA_TRY(err, cudaSetDevice(device));
+  const int64_t n = block->num_rows;
+  // ---- type inference over the postfix program
+  EvalParams p;
+  memset(&p, 0, sizeof(p));
+  int col_dtype[16];
+  bool col_nullable[16];
+  for (int c = 0; c < block->num_cols; ++c) {
+    col_dtype[c] = block->cols[c].dtype;
+    col_nullable[c] = block->cols[c].validity != nullptr || (block->cols[c].is_const && block->cols[c].konst.is_null);
+  }
+  int ot = 0;
+  bool o_nullable = false;
+  DBX_TRY(infer_expr_types(*expr, block->num_cols, col_dtype, col_nullable, p.nodes, &ot, &o_nullable, err));
   if (out_dtype) *out_dtype = ot | (o_nullable ? DBX_NULLABLE : 0);
 
   cudaStream_t st = nullptr;

@@ -1,9 +1,11 @@
-// eval_kernels.cuh — device side of dbx_eval_scalar: value images, the reference's cast / arithmetic
-// rules per expression node, and the two kernels built from them:
-//   eval_kernel           interprets the postfix program per row (value stack in registers);
-//   dbx_jit_eval (NVRTC)  the same per-node functions called with COMPILE-TIME node descriptions in a
-//                         generated straight-line body (eval.cu: specialise_expr) — the interpreter's
-//                         dispatch, type switches and stack traffic fold away.
+// eval_kernels.cuh — device side of dbx_eval_scalar: value images and the reference's cast / arithmetic
+// rules per expression node.  Three kinds of kernel are built from them:
+//   eval_kernel (eval.cu)  interprets the postfix program per row (value stack in registers);
+//   dbx_jit_eval (NVRTC)   the same per-node functions called with COMPILE-TIME node descriptions in a
+//                          generated straight-line body (eval.cu: specialised_source) — the interpreter's
+//                          dispatch, type switches and stack traffic fold away;
+//   the aggregate / filter kernels (agg_kernels.cuh: eval_computed) evaluate computed columns in
+//                          registers between their column loads and the table update.
 // Reference semantics: see eval.cu's header.
 #pragma once
 #include "common.cuh"
@@ -260,33 +262,16 @@ __device__ __forceinline__ void store_result(const EvalParams& p, int64_t r, uin
 }
 
 #ifndef DBX_JIT
-// The interpreter: an 8-deep value stack held in registers (push / pop shift the registers, so no
-// dynamically indexed local array), top of stack in s0.
-__global__ void __launch_bounds__(256) eval_kernel(const __grid_constant__ EvalParams p) {
-  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows; r += (int64_t)gridDim.x * blockDim.x) {
-    uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0;
-    bool n0 = false, n1 = false, n2 = false, n3 = false, n4 = false, n5 = false, n6 = false, n7 = false;
-    int err = 0;
-    for (int i = 0; i < p.n_nodes; ++i) {
-      const NodeDev& nd = p.nodes[i];
-      if (nd.kind == DBX_EXPR_COLUMN || nd.kind == DBX_EXPR_CONST) {
-        s7 = s6; s6 = s5; s5 = s4; s4 = s3; s3 = s2; s2 = s1; s1 = s0;
-        n7 = n6; n6 = n5; n5 = n4; n4 = n3; n3 = n2; n2 = n1; n1 = n0;
-        if (nd.kind == DBX_EXPR_COLUMN) load_column(p.cols[nd.col], r, nd.out, s0, n0);
-        else { s0 = nd.c_bits; n0 = !nd.c_null; }
-      } else if (nd.kind == DBX_EXPR_CAST) {
-        apply_cast(nd, s0, n0, err);
-      } else if (nd.func == DBX_FN_NOT || nd.func == DBX_FN_NEGATE || nd.func == DBX_FN_IS_NULL || nd.func == DBX_FN_IS_NOT_NULL) {
-        apply_unary(nd, s0, n0, err);
-      } else {
-        apply_binary(nd, s1, n1, s0, n0, err);  // s1 op s0 -> s1, then pop
-        s0 = s1; s1 = s2; s2 = s3; s3 = s4; s4 = s5; s5 = s6; s6 = s7;
-        n0 = n1; n1 = n2; n2 = n3; n3 = n4; n4 = n5; n5 = n6; n6 = n7;
-      }
-    }
-    store_result(p, r, s0, n0, err);
-  }
-}
+// The reference's type inference over a postfix program (arithmetics_type.rs): fills nodes[i] (types of
+// every node; COLUMN nodes keep the column index in `col`) and the result type and nullability.  Columns
+// are described by their dtype and nullability; `what` prefixes the error messages.  Shared by
+// dbx_eval_scalar and by the aggregate / filter operators' computed columns (agg.cu).
+int32_t infer_expr_types(const dbx_expr& expr, int n_cols, const int* col_dtype, const bool* col_nullable, NodeDev* nodes,
+                         int* out_dtype, bool* out_nullable, ErrorSink& err);
+// true when evaluating the (type-checked) program can raise on a row whose arguments are non-NULL:
+// `/`, `div` or `%` whose divisor is not a non-zero constant, a non-try cast that can overflow, or a
+// negation of an Int64 / UInt64
+bool expr_can_raise(const NodeDev* nodes, int n_nodes);
 #endif
 
 }  // namespace dbx

@@ -3,6 +3,7 @@
 // dbx_agg_params / dbx_predicate (include/dbx.h), passed BY VALUE to the kernels.
 #pragma once
 #include "common.cuh"
+#include "eval_kernels.cuh"
 
 namespace dbx {
 
@@ -10,6 +11,8 @@ constexpr int kMaxSlots = 8;    // distinct input columns one kernel reads
 constexpr int kMaxUpdates = 16; // state-word updates per passing row
 constexpr int kMaxWords = 15;   // state words per group (entry = key + words)
 constexpr int kMaxPairs = 2;    // 16-byte pairs of additive state words updated by ONE TMA bulk reduction
+constexpr int kMaxComputed = DBX_MAX_COMPUTED_COLS;  // computed columns one operator evaluates
+constexpr int kMaxCompNodes = 32;                    // postfix nodes of all its computed columns together
 
 // x % d for a runtime-constant divisor without a hardware divide: Granlund–Montgomery
 // round-up method (N = 64):  m' = floor(2^64 (2^l - d) / d) + 1,
@@ -168,6 +171,15 @@ struct KeyPartDev {
   uint64_t mask;       // value field mask (unshifted)
 };
 
+// One computed column (dbx_op_create_computed): the postfix program cnodes[first, first + n_nodes)
+// evaluated per row with eval_kernels.cuh's node functions; COLUMN nodes name a SLOT (NodeDev::col),
+// the value goes to slot `slot` as the 64-bit image load_slot would give a column of its type.
+struct CompDev {
+  int32_t first, n_nodes;
+  int32_t slot;
+  int32_t pad;
+};
+
 struct AggKernelParams {
   DevCol cols[kMaxSlots];
   PredNodeDev nodes[DBX_MAX_PRED_NODES];
@@ -192,6 +204,15 @@ struct AggKernelParams {
   int32_t ring_nsv;                 // number of stored slot arrays
   int8_t ring_sidx[kMaxSlots];      // slot -> storage index, -1: not stored
   int32_t hot_cache;                // 1: per-CTA shared-memory cache of hot groups (skewed keys), flushed at kernel end
+  // computed columns (kept behind every field above, so plans without them see the same layout):
+  // comp[0, comp_pred) feed the predicate and are evaluated before it, comp[comp_pred, n_comp) after it
+  int32_t n_comp, comp_pred;
+  uint32_t fresh_slots;             // slots that hold a computed value only (no input column is loaded into them)
+  int32_t pad_comp;
+  CompDev comp[kMaxComputed];
+  NodeDev cnodes[kMaxCompNodes];
+  int64_t expr_row0;                // number (since create / reset) of the row this launch's row 0 stands for
+  unsigned long long* expr_err;     // min over failing selected rows of (row << 8 | code); nullptr: the plan cannot raise
 };
 
 // The plan fields the fused kernels read per row, as ONE constexpr object: a run-time specialised
@@ -202,6 +223,13 @@ struct StaticPlan {
   PredNodeDev nodes[DBX_MAX_PRED_NODES];
   UpdateDev upd[kMaxUpdates];
   KeyPartDev key_parts[DBX_MAX_GROUP_COLS];
+  // computed columns, last: agg_jit_plan_text writes them only when there are some, so the text of every
+  // other plan (and the kernel compiled from it) does not change
+  int32_t n_comp, comp_pred;
+  uint32_t fresh_slots;
+  int32_t raises;                   // 1: a computed column after the predicate can raise (errors are recorded)
+  CompDev comp[kMaxComputed];
+  NodeDev cnodes[kMaxCompNodes];
 };
 
 }  // namespace dbx

@@ -325,9 +325,11 @@ int32_t pull_owned_block(std::unique_ptr<OwnedBlock>& result_dev, int device, cu
 
 
 // factories implemented next to each operator
-Op* make_agg_partial_op(const dbx_agg_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
-Op* make_agg_final_op(const dbx_agg_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
-Op* make_filter_op(const dbx_predicate* p, const int32_t* types, int32_t n, int device, int32_t* st);
+Op* make_agg_partial_op(const dbx_agg_params* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device,
+                        int32_t* st);
+Op* make_agg_final_op(const dbx_agg_params* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device,
+                      int32_t* st);
+Op* make_filter_op(const dbx_predicate* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device, int32_t* st);
 Op* make_topk_op(const dbx_topk_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
 Op* make_join_op(const dbx_join_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
 
@@ -406,7 +408,19 @@ int32_t dbx_device_synchronize(int32_t device) {
 
 int32_t dbx_op_create(int32_t kind, const void* params, const int32_t* input_types, int32_t n_input_cols,
                       int32_t device, dbx_op** out) {
+  return dbx_op_create_computed(kind, params, input_types, n_input_cols, nullptr, 0, device, out);
+}
+
+int32_t dbx_op_create_computed(int32_t kind, const void* params, const int32_t* input_types, int32_t n_input_cols,
+                               const dbx_expr* computed, int32_t n_computed, int32_t device, dbx_op** out) {
   if (!out || !params) { g_create_error.set("dbx_op_create: null argument"); return DBX_ERR_INVALID; }
+  if (n_computed < 0 || n_computed > DBX_MAX_COMPUTED_COLS) { g_create_error.set("dbx_op_create_computed: n_computed outside 0 .. DBX_MAX_COMPUTED_COLS"); return DBX_ERR_INVALID; }
+  if (n_computed > 0 && !computed) { g_create_error.set("dbx_op_create_computed: null computed list"); return DBX_ERR_INVALID; }
+  if (n_computed > 0 && n_input_cols + n_computed > 64) { g_create_error.set("dbx_op_create_computed: more than 64 input and computed columns"); return DBX_ERR_INVALID; }
+  if (n_computed > 0 && (kind == DBX_OP_TOPK || kind == DBX_OP_JOIN)) {
+    g_create_error.set("dbx_op_create_computed: computed columns are taken by the filter and aggregate operators only");
+    return DBX_ERR_UNSUPPORTED;
+  }
   *out = nullptr;
   int32_t ndev = 0;
   DBX_TRY(dbx_device_count(&ndev));
@@ -414,9 +428,9 @@ int32_t dbx_op_create(int32_t kind, const void* params, const int32_t* input_typ
   int32_t st = DBX_OK;
   Op* op = nullptr;
   switch (kind) {
-    case DBX_OP_AGG_PARTIAL: op = make_agg_partial_op((const dbx_agg_params*)params, input_types, n_input_cols, device, &st); break;
-    case DBX_OP_AGG_FINAL: op = make_agg_final_op((const dbx_agg_params*)params, input_types, n_input_cols, device, &st); break;
-    case DBX_OP_FILTER: op = make_filter_op((const dbx_predicate*)params, input_types, n_input_cols, device, &st); break;
+    case DBX_OP_AGG_PARTIAL: op = make_agg_partial_op((const dbx_agg_params*)params, input_types, n_input_cols, computed, n_computed, device, &st); break;
+    case DBX_OP_AGG_FINAL: op = make_agg_final_op((const dbx_agg_params*)params, input_types, n_input_cols, computed, n_computed, device, &st); break;
+    case DBX_OP_FILTER: op = make_filter_op((const dbx_predicate*)params, input_types, n_input_cols, computed, n_computed, device, &st); break;
     case DBX_OP_TOPK: op = make_topk_op((const dbx_topk_params*)params, input_types, n_input_cols, device, &st); break;
     case DBX_OP_JOIN: op = make_join_op((const dbx_join_params*)params, input_types, n_input_cols, device, &st); break;
     default: g_create_error.set("dbx_op_create: unknown operator kind"); return DBX_ERR_INVALID;
@@ -436,10 +450,14 @@ int32_t dbx_op_destroy(dbx_op* op) {
   return DBX_OK;
 }
 
-#define DBX_OP_ENTER(op)                                                       \
+#define DBX_OP_ENTER_ANY(op)                                                   \
   if (!(op)) return DBX_ERR_INVALID;                                           \
   Op* o = reinterpret_cast<Op*>(op);                                           \
   DBX_CUDA_TRY(o->err, cudaSetDevice(o->device));
+// a poisoned handle (its input failed to evaluate) takes reset and destroy only
+#define DBX_OP_ENTER(op)                                                       \
+  DBX_OP_ENTER_ANY(op)                                                         \
+  if (o->poisoned) { o->err.set("the operator's input failed to evaluate (" + o->poison_msg + "): reset it"); return DBX_ERR_STATE; }
 
 int32_t dbx_op_push(dbx_op* op, const dbx_block* block) {
   DBX_OP_ENTER(op);
@@ -461,9 +479,9 @@ int32_t dbx_op_pull(dbx_op* op, int32_t out_mem, dbx_block* out, int32_t* has_bl
   return o->pull(out_mem, out, has_block);
 }
 int32_t dbx_op_reset(dbx_op* op) {
-  DBX_OP_ENTER(op);
+  DBX_OP_ENTER_ANY(op);
   int32_t st = o->reset();
-  if (st == DBX_OK) o->finished = false;
+  if (st == DBX_OK) { o->finished = false; o->poisoned = false; }
   return st;
 }
 int32_t dbx_block_release(dbx_block* block) {

@@ -158,6 +158,10 @@ class Op {
   int32_t timing_end();
   bool timed = false;
   bool finished = false;
+  // an evaluation error of the pushed input: every call but reset / destroy fails until reset
+  bool poisoned = false;
+  std::string poison_msg;
+  void poison(const std::string& m) { poisoned = true; poison_msg = m; err.set(m); }
 };
 
 // Converts a scalar to the 64-bit image the kernels use for its class (i64 / u64 / f64 bits).

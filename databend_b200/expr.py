@@ -65,6 +65,7 @@ class Node:
 
 
 def compare(op: int, lhs: Operand, rhs: Operand) -> Node:
+    """An operand may also be a numeric scalar_expr.SExpr: the operator evaluates it as a computed column."""
     return Node(abi.PRED_CMP, cmp=op, lhs=lhs, rhs=rhs)
 
 
@@ -84,7 +85,8 @@ def or_(*children: Node) -> Node:
     return Node(abi.PRED_OR, children=list(children))
 
 
-def bool_column(index: int) -> Node:
+def bool_column(index) -> Node:
+    """A Boolean input column, or a Boolean scalar_expr.SExpr (a computed column)."""
     return Node(abi.PRED_BOOLCOL, value=index)
 
 
@@ -92,8 +94,12 @@ def bool_scalar(v: bool) -> Node:
     return Node(abi.PRED_CONST, value=int(v))
 
 
-def _operand(o: Operand) -> abi.Operand:
+def _operand(o: Operand, computed=None) -> abi.Operand:
     c = abi.Operand()
+    if not isinstance(o, (Literal, ColumnRef)):  # scalar_expr.SExpr: its computed column
+        c.is_const = 0
+        c.col = _computed_col(o, computed)
+        return c
     if isinstance(o, Literal):
         c.is_const = 1
         c.c = make_scalar(o.dtype, o.value)
@@ -106,8 +112,29 @@ def _operand(o: Operand) -> abi.Operand:
     return c
 
 
-def build_predicate(root: Optional[Node]) -> abi.Predicate:
-    """Post-order flattening into dbx_predicate."""
+def _computed_col(e, computed) -> int:
+    if computed is None:
+        raise ValueError("a predicate with scalar expressions needs the operator's computed-column list")
+    return computed.column(e)
+
+
+def sexprs(root: Optional[Node]):
+    """The scalar expressions (computed columns) a predicate uses, in order."""
+    if root is None:
+        return []
+    out = []
+    if root.kind == abi.PRED_CMP:
+        out += [o for o in (root.lhs, root.rhs) if not isinstance(o, (Literal, ColumnRef))]
+    elif root.kind == abi.PRED_BOOLCOL and not isinstance(root.value, int):
+        out.append(root.value)
+    for ch in root.children or []:
+        out += sexprs(ch)
+    return out
+
+
+def build_predicate(root: Optional[Node], computed=None) -> abi.Predicate:
+    """Post-order flattening into dbx_predicate.  `computed` (scalar_expr.Computed) numbers the
+    scalar expressions the predicate uses."""
     p = abi.Predicate()
     p.n_nodes = 0
     if root is None:
@@ -122,10 +149,10 @@ def build_predicate(root: Optional[Node]) -> abi.Predicate:
         pn = abi.PredNode()
         pn.kind = n.kind
         pn.cmp = n.cmp
-        pn.value = n.value
+        pn.value = n.value if isinstance(n.value, int) else _computed_col(n.value, computed)
         if n.kind == abi.PRED_CMP:
-            pn.lhs = _operand(n.lhs)
-            pn.rhs = _operand(n.rhs)
+            pn.lhs = _operand(n.lhs, computed)
+            pn.rhs = _operand(n.rhs, computed)
         if n.children:
             pn.n_children = len(n.children)
         out.append(pn)

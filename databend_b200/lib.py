@@ -109,6 +109,8 @@ def load():
         "dbx_runtime_filter_export": (i32, [vp, i32, P(C.c_uint32), i64, P(i64), i64]),
         "dbx_runtime_filter_apply": (i32, [vp, P(abi.Block), P(i32), i32, P(abi.Block), P(i64)]),
         "dbx_runtime_filter_destroy": (i32, [vp]),
+        "dbx_op_create_computed": (i32, [i32, vp, P(i32), i32, P(abi.Expr), i32, i32, P(vp)]),
+        "dbx_agg_expr_jit_selftest": (i32, [C.c_char_p, i32]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)  # AttributeError = the library does not export a declared symbol

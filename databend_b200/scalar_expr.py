@@ -84,6 +84,37 @@ def flatten(e: SExpr) -> abi.Expr:
     return out
 
 
+def key(e: SExpr) -> tuple:
+    """Structural identity of an expression (equal keys: one computed column)."""
+    return (e.kind, e.func, e.col, e.dtype, repr(e.value), e.try_cast, tuple(key(a) for a in e.args))
+
+
+class Computed:
+    """The distinct expressions an operator evaluates, numbered after its input columns in first-use order
+    (column n_inputs + i is exprs[i])."""
+
+    def __init__(self, n_inputs: int):
+        self.n_inputs = n_inputs
+        self.exprs: List[SExpr] = []
+        self._index = {}
+
+    def column(self, e) -> int:
+        """Column index of an input index or an SExpr (added on first use)."""
+        if not isinstance(e, SExpr):
+            return e
+        k = key(e)
+        if k not in self._index:
+            self._index[k] = self.n_inputs + len(self.exprs)
+            self.exprs.append(e)
+        return self._index[k]
+
+    def to_c(self):
+        arr = (abi.Expr * max(1, len(self.exprs)))()
+        for i, e in enumerate(self.exprs):
+            arr[i] = flatten(e)
+        return arr
+
+
 class EvalError(DbxError):
     def __init__(self, status, message, row):
         super().__init__(status, message)

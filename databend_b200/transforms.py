@@ -16,12 +16,13 @@ transform()/on_finish() directly (the adaptor contract of transform_accumulating
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from . import abi, expr as E
+from . import abi, expr as E, scalar_expr as S
 from .block import Column, DataBlock, np_dtype
 from .lib import DbxError, check, load
 
@@ -128,11 +129,16 @@ def _block_from_c(b: abi.Block, device: int) -> DataBlock:
 class _Op:
     """Owns one dbx_op handle."""
 
-    def __init__(self, kind: int, params, input_types: Sequence[int], device: int):
+    def __init__(self, kind: int, params, input_types: Sequence[int], device: int, computed=None):
         self._h = C.c_void_p()
         self.device = device
         types = (C.c_int32 * max(1, len(input_types)))(*input_types)
         self._params = params
+        if computed is not None and computed.exprs:
+            self._computed = computed.to_c()
+            check(load().dbx_op_create_computed(kind, C.cast(C.byref(params), C.c_void_p), types, len(input_types), self._computed,
+                                                len(computed.exprs), device, C.byref(self._h)))
+            return
         check(load().dbx_op_create(kind, C.cast(C.byref(params), C.c_void_p), types, len(input_types), device,
                                    C.byref(self._h)))
 
@@ -198,7 +204,9 @@ class TransformFilter(_Op):
     true, in input order, for every column.  NULL predicate values count as false."""
 
     def __init__(self, predicate: Optional[E.Node], input_types: Sequence[int], device: int = 0):
-        super().__init__(abi.OP_FILTER, E.build_predicate(predicate), input_types, device)
+        """Predicate operands may be scalar_expr.SExpr: evaluated inside the filter kernel."""
+        computed = S.Computed(len(input_types))
+        super().__init__(abi.OP_FILTER, E.build_predicate(predicate, computed), input_types, device, computed)
 
     def transform(self, block: DataBlock) -> DataBlock:
         self.push(block)
@@ -216,18 +224,40 @@ class AggregatorParams:
     aggregate_functions: List[Tuple[str, Optional[int]]]
     expected_groups: int = 0
 
-    def to_c(self, filter_expr: Optional[E.Node] = None) -> abi.AggParams:
+    # A group column or an aggregate argument may also be a scalar_expr.SExpr: the operators evaluate it
+    # as a computed column inside their kernels.
+
+    def computed(self, n_inputs: int, filter_expr: Optional[E.Node] = None) -> S.Computed:
+        """The operator's computed columns: the expressions of the group columns and arguments first (so a
+        final operator built from the same params numbers them alike), then the predicate's."""
+        c = S.Computed(n_inputs)
+        for g in self.group_columns:
+            c.column(g)
+        for _, arg in self.aggregate_functions:
+            if arg is not None:
+                c.column(arg)
+        for e in E.sexprs(filter_expr):
+            c.column(e)
+        return c
+
+    def to_c(self, filter_expr: Optional[E.Node] = None, computed: Optional[S.Computed] = None) -> abi.AggParams:
+        def colno(x):
+            if isinstance(x, S.SExpr):
+                if computed is None:
+                    raise ValueError("parameters with scalar expressions need the operator's computed-column list")
+                return computed.column(x)
+            return x
         p = abi.AggParams()
         p.n_group_cols = len(self.group_columns)
         for i, g in enumerate(self.group_columns):
-            p.group_cols[i] = g
+            p.group_cols[i] = colno(g)
         p.n_aggs = len(self.aggregate_functions)
         for i, (name, arg) in enumerate(self.aggregate_functions):
             if name not in _AGG_NAMES:
                 raise DbxError(abi.ERR_UNSUPPORTED, f"Unknown aggregate function {name}")  # factory.get error
             p.aggs[i].kind = _AGG_NAMES[name]
-            p.aggs[i].arg_col = -1 if arg is None else arg
-        p.filter = E.build_predicate(filter_expr)
+            p.aggs[i].arg_col = -1 if arg is None else colno(arg)
+        p.filter = E.build_predicate(filter_expr, computed)
         p.expected_groups = self.expected_groups
         return p
 
@@ -256,11 +286,22 @@ class TransformPartialAggregate(_Op):
     def __init__(self, params: AggregatorParams, input_types: Sequence[int], filter_expr: Optional[E.Node] = None,
                  device: int = 0):
         self.params = params
-        super().__init__(abi.OP_AGG_PARTIAL, params.to_c(filter_expr), input_types, device)
+        computed = params.computed(len(input_types), filter_expr)
+        super().__init__(abi.OP_AGG_PARTIAL, params.to_c(filter_expr, computed), input_types, device, computed)
 
     def transform(self, block: DataBlock) -> List[DataBlock]:
         self.push(block)
         return []
+
+    def finish(self):
+        """A computed column that failed on a row the predicate kept raises scalar_expr.EvalError with
+        the first failing row (rows counted from the first row pushed since create / reset)."""
+        st = load().dbx_op_finish(self._h)
+        if st == abi.ERR_BAD_ARGUMENTS:
+            msg = (load().dbx_last_error(self._h) or b"").decode("utf-8", "replace")
+            m = re.search(r"first failing row (\d+)", msg)
+            raise S.EvalError(st, msg, int(m.group(1)) if m else -1)
+        check(st, self._h)
 
     def on_finish(self):
         self.finish()
@@ -279,7 +320,8 @@ class TransformPartialAggregate(_Op):
 class TransformFinalAggregate(_Op):
     def __init__(self, params: AggregatorParams, input_types: Sequence[int], device: int = 0):
         self.params = params
-        super().__init__(abi.OP_AGG_FINAL, params.to_c(None), input_types, device)
+        computed = params.computed(len(input_types))
+        super().__init__(abi.OP_AGG_FINAL, params.to_c(None, computed), input_types, device, computed)
 
     def transform(self, partial: TransformPartialAggregate) -> List[DataBlock]:
         """handle_meta -> combine_payload (transform_aggregate_final.rs:201-303)."""

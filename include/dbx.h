@@ -308,6 +308,46 @@ int32_t dbx_op_synchronize(dbx_op* op);
  * reuse pinned-host / device input buffers (the Arc<Buffer> of the reference can be dropped). */
 int32_t dbx_op_inputs_consumed(dbx_op* op);
 
+/* Computed columns: dbx_op_create with scalar expressions evaluated inside the operator's kernels
+ * (the EvalScalar the reference places between the filtered input and the Aggregate,
+ * binder/aggregate.rs:1100-1143, fused into the scan).  computed[i] is a dbx_expr (see dbx_eval_scalar)
+ * over the INPUT columns and becomes column n_input_cols + i.  Wherever `params` take a column index
+ * (group_cols, aggs[].arg_col, predicate operands and BOOLCOL), that index may name a computed column,
+ * which is accepted wherever an input column of the same type and nullability is accepted, and refused
+ * wherever such a column is refused.
+ *   Kinds: DBX_OP_FILTER, DBX_OP_AGG_PARTIAL (with or without GROUP BY) and DBX_OP_AGG_FINAL (which
+ *   evaluates nothing: the list only fixes its argument, result and spill types; create it with the
+ *   partial's list).  DBX_OP_TOPK / DBX_OP_JOIN with n_computed > 0: DBX_ERR_UNSUPPORTED.
+ *   n_computed == 0 is dbx_op_create.
+ *   Types: dbx_eval_scalar's inference.  Nullability comes from the schema: the DBX_NULLABLE flags of
+ *   input_types, try_cast and NULL literals (never from a pushed block's validity).
+ *   DBX_ERR_INVALID: a computed expression that references a computed column or a column outside the
+ *   input schema, n_computed outside 0 .. DBX_MAX_COMPUTED_COLS, n_input_cols + n_computed > 64.
+ *   DBX_ERR_UNSUPPORTED: a plan that needs more than 8 values per row after computed columns took the
+ *   slots of inputs whose last use precedes them.
+ * Semantics follow the plan order Filter -> EvalScalar -> Aggregate:
+ *   - Aggregate arguments and GROUP BY expressions are evaluated on the rows the predicate keeps only.
+ *     A row raises ("Division by zero", "divided by zero", "number overflowed") only if the predicate
+ *     keeps it and the failing call's own arguments are non-NULL (passthrough_nullable).
+ *   - A computed column the predicate uses must not be able to raise: one containing `/`, `div` or `%`
+ *     whose divisor is not a non-zero constant, a non-try cast that can overflow, or a negation of an
+ *     Int64 / UInt64 is refused with DBX_ERR_UNSUPPORTED.  The reference's selector evaluates AND / OR
+ *     children under an adaptive permutation (expression/src/filter/selector.rs:182-300), so which rows
+ *     reach such an expression there is not deterministic.
+ *   - Pushes stay asynchronous.  A plan whose expressions can raise keeps a device word, the minimum of
+ *     (row << 8 | code) over failing rows, rows counted from the first row pushed since create or reset;
+ *     dbx_op_finish synchronises for such plans only and returns DBX_ERR_BAD_ARGUMENTS with the
+ *     reference's message and the first failing row in dbx_last_error; so does every call that hands the
+ *     partial's state on without a finish (dbx_agg_final_merge_partial, dbx_agg_partial_partition /
+ *     _serialize, dbx_agg_exchange_scatter).  After that every call but
+ *     dbx_op_reset and dbx_op_destroy returns DBX_ERR_STATE, so no result built from the failed input
+ *     leaves the operator.  DBX_OP_FILTER never raises (its computed columns feed the predicate only).
+ *     Plans whose expressions cannot raise keep an asynchronous finish. */
+#define DBX_MAX_COMPUTED_COLS 4
+typedef struct dbx_expr dbx_expr;
+int32_t dbx_op_create_computed(int32_t kind, const void* params, const int32_t* input_types, int32_t n_input_cols,
+                               const dbx_expr* computed, int32_t n_computed, int32_t device, dbx_op** out);
+
 /* Join probe side: Join::probe_block(block) -> JoinStream::next()* ; output blocks are
  * pulled with dbx_op_pull until drained. */
 int32_t dbx_join_probe(dbx_op* op, const dbx_block* block);
@@ -512,11 +552,11 @@ typedef struct dbx_expr_node {
   dbx_scalar c;     /* DBX_EXPR_CONST */
 } dbx_expr_node;
 #define DBX_MAX_EXPR_NODES 32
-typedef struct dbx_expr {
+struct dbx_expr {
   int32_t n_nodes;
   int32_t reserved;
   dbx_expr_node nodes[DBX_MAX_EXPR_NODES];
-} dbx_expr;
+};
 /* out: library-owned block with ONE column (dbx_block_release); *out_dtype = its dbx_dtype
  * (| DBX_NULLABLE).  A per-row evaluation error returns DBX_ERR_BAD_ARGUMENTS with the reference's
  * message in dbx_last_error(NULL) and the first failing row in *first_error_row. */
@@ -579,6 +619,9 @@ int32_t dbx_agg_jit_selftest(char* msg, int32_t msg_cap);
 /* Same for the scalar-expression evaluator: generates and compiles the straight-line kernel of a canned
  * expression (dbx_eval_scalar compiles one per expression shape; DBX_EVAL_JIT=0 keeps the interpreter). */
 int32_t dbx_eval_jit_selftest(char* msg, int32_t msg_cap);
+/* Same for the aggregate kernels with computed columns: compiles a canned Q1-shaped plan (two computed
+ * slots that take the slots of inputs whose last use precedes them) and checks all four entries. */
+int32_t dbx_agg_expr_jit_selftest(char* msg, int32_t msg_cap);
 /* Stream of a handle as a cudaStream_t value (for external event timing). */
 int32_t dbx_op_stream(dbx_op* op, void** stream);
 

@@ -10,6 +10,8 @@
 // src/common/base/src/base/ordered_float.rs:147-201); ties are broken by ascending row id, as in
 // the oracle.  Everything below is hand-written (no CUB):
 //
+//   several keys, LIMIT k the same streaming top-k on a composite order image of all keys (W <= 5
+//   (k <= 4 Mi)           64-bit words, see "streaming top-k over several keys" below)
 //   LIMIT k (k <= 4 Mi)   streaming top-k: the column is read ONCE (8 B/row, 256-bit streaming
 //                         loads); a row survives only if it beats the boundary (the k-th best key
 //                         so far — the reference's TopN boundary filter), kept in DEVICE memory and
@@ -498,6 +500,458 @@ __global__ void sort_emit_kernel(const __grid_constant__ SortEmitArgs a) {
   }
 }
 
+// ================================================================ streaming top-k over several keys
+// ORDER BY k0, k1, ... LIMIT k runs the same candidate list / boundary / cut machinery as one key,
+// on a composite order image: every row's keys packed into one big-endian unsigned integer of W
+// 64-bit words whose lexicographic order is the ORDER BY order (the reference builds the same thing
+// as a byte-comparable row encoding, sorts/core/row_convert/fixed_encode.rs:22-57).  Per key, most
+// significant first:
+//   nullable key   one placement bit: NULLS FIRST: NULL 0, valid 1; NULLS LAST: NULL 1, valid 0
+//   value          the key's natural width (8/16/32/64 bits); signed integers with the sign bit
+//                  flipped, floats as their OrderedFloat image (-0 == +0, every NaN greatest),
+//                  complemented for DESC; 0 on a NULL row, so NULL rows tie and later keys decide
+// Fields may straddle words: the image is only compared, never decoded.  4 x 65 bits: W <= 5.
+constexpr int kMaxImageWords = 5;
+enum : int { MST_NULLS = 3, MST_BOUND = ST_WORDS };  // multi-key state: [count, -, overflow, nulls emitted, boundary[W]]
+
+struct MultiKeys {
+  DevCol col[DBX_MAX_SORT_KEYS];      // col[0] is the first key
+  int32_t off[DBX_MAX_SORT_KEYS];     // bit offset of the key's first field, from the image's top bit
+  int32_t width[DBX_MAX_SORT_KEYS];   // value field bits
+  int32_t nullable[DBX_MAX_SORT_KEYS];
+  int32_t nulls_first[DBX_MAX_SORT_KEYS];
+  int32_t asc[DBX_MAX_SORT_KEYS];
+  int32_t n_keys;
+  int32_t lead_bits;  // bits taken by the first key (placement bit + value): <= 65
+};
+
+// Host side of the layout: field offsets per key and the number of image words.
+inline int multi_key_layout(const int* dtypes, const bool* nullable, int n_keys, MultiKeys* mk) {
+  int bit = 0;
+  for (int k = 0; k < n_keys; ++k) {
+    mk->off[k] = bit;
+    mk->nullable[k] = nullable[k] ? 1 : 0;
+    mk->width[k] = 8 * dtype_size(dtypes[k]);
+    bit += mk->nullable[k] + mk->width[k];
+    if (k == 0) mk->lead_bits = bit;
+  }
+  mk->n_keys = n_keys;
+  return (bit + 63) / 64;
+}
+
+// The value field of one key (widened bits as load_widened returns them), `width` bits wide.
+__device__ __forceinline__ uint64_t key_field(uint64_t v, int dtype, int width, bool asc) {
+  const uint64_t mask = width == 64 ? ~0ULL : (1ULL << width) - 1;
+  uint64_t o;
+  if (dtype == DBX_F64) {
+    double d = __longlong_as_double((long long)v);
+    if (d == 0.0) d = 0.0;  // -0 == +0
+    o = f64_to_ordered(d);
+  } else if (dtype == DBX_F32) {  // the same order as the widened value
+    float f = (float)__longlong_as_double((long long)v);
+    uint32_t u;
+    if (f != f) u = 0xFFFFFFFFu;
+    else {
+      if (f == 0.0f) f = 0.0f;
+      u = __float_as_uint(f);
+      u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    }
+    o = u;
+  } else if (dtype == DBX_I8 || dtype == DBX_I16 || dtype == DBX_I32 || dtype == DBX_I64) {
+    o = (v ^ (1ULL << (width - 1))) & mask;
+  } else {
+    o = v & mask;
+  }
+  return asc ? o : o ^ mask;
+}
+
+// OR the `wd`-bit value v into the image at bit `off` (counted from the top bit of word 0)
+template <int W>
+__device__ __forceinline__ void img_put(uint64_t (&img)[W], int off, int wd, uint64_t v) {
+  const int w0 = off >> 6, end = (off & 63) + wd;  // end <= 128
+#pragma unroll
+  for (int w = 0; w < W; ++w) {
+    if (w == w0) img[w] |= end <= 64 ? v << (64 - end) : v >> (end - 64);
+    if (w == w0 + 1 && end > 64) img[w] |= v << (128 - end);
+  }
+}
+
+template <int W>
+__device__ __forceinline__ void img_put_key(const MultiKeys& mk, int k, bool ok, uint64_t v, uint64_t (&img)[W]) {
+  int off = mk.off[k];
+  if (mk.nullable[k]) { img_put(img, off, 1, (uint64_t)(ok == (mk.nulls_first[k] != 0))); ++off; }
+  if (ok) img_put(img, off, mk.width[k], key_field(v, mk.col[k].dtype, mk.width[k], mk.asc[k] != 0));
+}
+
+template <int W>
+__device__ __forceinline__ bool img_le(const uint64_t (&a)[W], const uint64_t (&b)[W]) {
+#pragma unroll
+  for (int w = 0; w < W; ++w)
+    if (a[w] != b[w]) return a[w] < b[w];
+  return true;
+}
+
+// The image of row r (first key already loaded: ok0, v0) if it can still be in the top k, i.e.
+// image <= boundary.  The first key's fields are compared first (bl0, bl1: the same bits of the
+// boundary); the later key columns are read only when they are not greater.
+template <int W>
+__device__ __forceinline__ bool multi_row(const MultiKeys& mk, int64_t r, bool ok0, uint64_t v0, const uint64_t (&bound)[W], uint64_t bl0,
+                                          uint64_t bl1, uint64_t pol, uint64_t (&img)[W]) {
+#pragma unroll
+  for (int w = 0; w < W; ++w) img[w] = 0;
+  img_put_key(mk, 0, ok0, v0, img);
+  if (img[0] > bl0) return false;
+  if (W > 1 && img[0] == bl0 && img[W > 1 ? 1 : 0] > bl1) return false;  // word 1 holds first-key bits only for a 65-bit key
+#pragma unroll
+  for (int k = 1; k < DBX_MAX_SORT_KEYS; ++k) {
+    if (k >= mk.n_keys) break;
+    const DevCol& c = mk.col[k];
+    const bool ok = !c.validity || bit_test(c.validity, c.vbit_off + r);
+    img_put_key(mk, k, ok, ok ? load_widened(c, r, pol) : 0, img);
+  }
+  return img_le(img, bound);
+}
+
+// One candidate list for all rows (NULL rows included: their placement bits order them).
+struct MultiList {
+  uint64_t* img;    // [W][cap]: image word w of entry i at img[w * cap + i]
+  uint64_t* rowid;  // global row ordinal
+  uint64_t* bits;   // the first key's original value bits (widened), 0 for NULL
+  unsigned long long* state;  // MST_* words
+  int64_t cap;
+};
+
+template <int W>
+__device__ __forceinline__ void mcand_append_warp(const MultiList& l, bool keep, const uint64_t (&img)[W], uint64_t rid, uint64_t b, int lane) {
+  const uint32_t bal = __ballot_sync(0xffffffffu, keep);
+  if (!bal) return;
+  unsigned long long base = 0;
+  if (lane == __ffs(bal) - 1) base = atomicAdd(&l.state[ST_COUNT], (unsigned long long)__popc(bal));
+  base = __shfl_sync(0xffffffffu, base, __ffs(bal) - 1);
+  if (keep) {
+    const unsigned long long pos = base + __popc(bal & ((1u << lane) - 1));
+    if ((int64_t)pos < l.cap) {
+#pragma unroll
+      for (int w = 0; w < W; ++w) l.img[w * l.cap + pos] = img[w];
+      l.rowid[pos] = rid;
+      l.bits[pos] = b;
+    } else {
+      l.state[ST_OVERFLOW] = 1;
+    }
+  }
+}
+
+// topk_scan_kernel for a composite image: the first key is read densely (FAST: 8-byte column, 32 B
+// aligned, no validity: 256-bit streaming loads with the next tile prefetched); a row whose first
+// key is beyond the boundary's is rejected without touching the other key columns.  Launched with
+// 256 threads; 80 registers (3 CTAs per SM) leave the W = 1 .. 5 instantiations without spills.
+template <int W, bool FAST>
+__global__ void __maxnreg__(80) topk_multi_scan_kernel(const __grid_constant__ MultiKeys mk, int64_t n, int64_t row_base,
+                                                              const __grid_constant__ MultiList cand) {
+  const uint64_t pol = make_policy_evict_first();
+  const int lane = threadIdx.x & 31;
+  uint64_t bound[W];
+#pragma unroll
+  for (int w = 0; w < W; ++w) bound[w] = cand.state[MST_BOUND + w];
+  const int lb = mk.lead_bits;
+  const uint64_t bl0 = bound[0] & (lb >= 64 ? ~0ULL : ~(~0ULL >> lb));
+  const uint64_t bl1 = W > 1 && lb > 64 ? bound[W > 1 ? 1 : 0] & 0x8000000000000000ULL : 0;
+  const DevCol& col = mk.col[0];
+  uint64_t img[W];
+  if (FAST) {
+    const int64_t n_tiles = n / 2048;
+    const char* base = (const char*)col.data;
+    u64x4 q0, q1;
+    q0.x = q0.y = q0.z = q0.w = q1.x = q1.y = q1.z = q1.w = 0;
+    int64_t tile = blockIdx.x;
+    if (tile < n_tiles) {
+      q0 = ld_stream_256(base + (tile * 2048 + 4 * (int64_t)threadIdx.x) * 8);
+      q1 = ld_stream_256(base + (tile * 2048 + 1024 + 4 * (int64_t)threadIdx.x) * 8);
+    }
+    for (; tile < n_tiles; tile += gridDim.x) {
+      __syncwarp();
+      const u64x4 c0 = q0, c1 = q1;
+      const int64_t nt = tile + gridDim.x;
+      if (nt < n_tiles) {
+        q0 = ld_stream_256(base + (nt * 2048 + 4 * (int64_t)threadIdx.x) * 8);
+        q1 = ld_stream_256(base + (nt * 2048 + 1024 + 4 * (int64_t)threadIdx.x) * 8);
+      }
+      const uint64_t v[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+      bool any = false;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {  // first key only (a non-nullable 64-bit key: one word)
+        const uint64_t f = key_field(v[j], col.dtype, 64, mk.asc[0] != 0);
+        any |= f <= bl0;
+      }
+      if (!__any_sync(0xffffffffu, any)) continue;  // the common case once the boundary is tight
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int64_t r = tile * 2048 + (j >> 2) * 1024 + 4 * (int64_t)threadIdx.x + (j & 3);
+        const bool keep = multi_row(mk, r, true, v[j], bound, bl0, bl1, pol, img);
+        mcand_append_warp(cand, keep, img, (uint64_t)(row_base + r), v[j], lane);
+      }
+    }
+  }
+  const int64_t first = FAST ? (n / 2048) * 2048 : 0;
+  const int64_t n_tiles = (n - first + 1023) / 1024;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    __syncwarp();
+    const int64_t r0 = first + tile * 1024 + 4 * (int64_t)threadIdx.x;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const bool in = r0 + j < n;
+      const bool ok = in && (!col.validity || bit_test(col.validity, col.vbit_off + r0 + j));
+      const uint64_t v = ok ? load_widened(col, r0 + j, pol) : 0;
+      bool keep = false;
+      if (in) keep = multi_row(mk, r0 + j, ok, v, bound, bl0, bl1, pol, img);
+      mcand_append_warp(cand, keep, img, (uint64_t)(row_base + r0 + j), v, lane);
+    }
+  }
+}
+
+// topk_cut_kernel over (W image words, row id): MSD 8-bit digit passes over 8 (W + 1) digits; the
+// loop ends as soon as the bucket that contains the k-th entry is taken whole.  Publishes the
+// k-th image (or an upper bound of it) as the W-word boundary.
+struct MultiCutArgs {
+  MultiList l;
+  uint64_t* alt_img;  // [W][k] scratch
+  uint64_t* alt_rowid;
+  uint64_t* alt_bits;
+  int64_t k;
+  int64_t threshold;
+};
+template <int E>
+__device__ __forceinline__ uint64_t word_at(const uint64_t (&e)[E], int q) {
+  uint64_t x = e[0];
+#pragma unroll
+  for (int w = 1; w < E; ++w)
+    if (q == w) x = e[w];
+  return x;
+}
+template <int W>
+__global__ void __launch_bounds__(1024) topk_multi_cut_kernel(const __grid_constant__ MultiCutArgs a) {
+  constexpr int E = W + 1;  // entry: image words, row id
+  constexpr int T = (kCutActive + 1023) / 1024;
+  __shared__ unsigned int s_hist[256];
+  __shared__ unsigned int s_pick[3];
+  __shared__ unsigned int s_out, s_nact;
+  extern __shared__ __align__(16) uint64_t s_cut_dyn[];  // active set: [E][kCutActive]
+  const MultiList& l = a.l;
+  const int64_t cnt = (int64_t)l.state[ST_COUNT];
+  const int64_t n = cnt < l.cap ? cnt : l.cap;
+  if (n <= a.threshold || n <= a.k) return;
+  const int tid = threadIdx.x, lane = tid & 31;
+  auto load_entry = [&](int64_t i, uint64_t (&e)[E]) {
+#pragma unroll
+    for (int w = 0; w < W; ++w) e[w] = l.img[w * l.cap + i];
+    e[W] = l.rowid[i];
+  };
+  uint64_t th[E];
+#pragma unroll
+  for (int w = 0; w < E; ++w) th[w] = 0;
+  int64_t k_rem = a.k;
+  bool closed = false;
+  bool in_smem = false;
+  int64_t n_act = n;
+  for (int p = 0; p < 8 * E && !closed; ++p) {
+    if (tid < 256) s_hist[tid] = 0;
+    if (tid == 0) s_nact = 0;
+    __syncthreads();
+    const int q = p >> 3, sh = 56 - 8 * (p & 7);
+    const uint64_t thq = word_at(th, q);
+    const bool gather = !in_smem && n_act <= kCutActive;
+    const int64_t n_scan = in_smem ? n_act : n;
+    for (int64_t i0 = tid - lane; i0 < n_scan; i0 += 1024) {
+      const int64_t i = i0 + lane;
+      bool m = i < n_scan;
+      int d = 0;
+      uint64_t e[E];
+#pragma unroll
+      for (int w = 0; w < E; ++w) e[w] = 0;
+      if (m) {
+        if (in_smem) {
+#pragma unroll
+          for (int w = 0; w < E; ++w) e[w] = s_cut_dyn[w * kCutActive + i];
+        } else {
+          load_entry(i, e);
+        }
+        const uint64_t eq = word_at(e, q);
+        if (!in_smem) {
+#pragma unroll
+          for (int w = 0; w < E; ++w)
+            if (w < q) m &= e[w] == th[w];
+          if ((p & 7) != 0) m &= (eq >> (sh + 8)) == (thq >> (sh + 8));
+        }
+        d = (int)((eq >> sh) & 255);
+      }
+      const unsigned mm = __ballot_sync(0xffffffffu, m);
+      if (!mm) continue;
+      if (gather) {
+        unsigned int base = 0;
+        if (lane == __ffs(mm) - 1) base = atomicAdd(&s_nact, (unsigned)__popc(mm));
+        base = __shfl_sync(0xffffffffu, base, __ffs(mm) - 1);
+        if (m) {
+          const unsigned int qq = base + __popc(mm & ((1u << lane) - 1));
+          if (qq < (unsigned)kCutActive) {
+#pragma unroll
+            for (int w = 0; w < E; ++w) s_cut_dyn[w * kCutActive + qq] = e[w];
+          }
+        }
+      }
+      const int d0 = __shfl_sync(0xffffffffu, d, __ffs(mm) - 1);
+      const unsigned same = __ballot_sync(0xffffffffu, m && d == d0);
+      if (same == mm) { if (lane == __ffs(mm) - 1) atomicAdd(&s_hist[d0], (unsigned)__popc(mm)); }
+      else if (m) atomicAdd(&s_hist[d], 1u);
+    }
+    __syncthreads();
+    cut_find_bucket(s_hist, k_rem, s_pick, tid);
+    __syncthreads();
+    const uint64_t bkt = s_pick[0];
+#pragma unroll
+    for (int w = 0; w < E; ++w)
+      if (w == q) th[w] |= bkt << sh;
+    k_rem -= s_pick[1];
+    if (gather || in_smem) {
+      // keep only the chosen bucket of the shared-memory set (gathered under the OLD prefix)
+      const int64_t n_have = n_act;  // <= kCutActive
+      in_smem = true;
+      if (tid == 0) s_out = 0;
+      __syncthreads();
+      uint64_t ke[T][E];
+      bool kk[T];
+#pragma unroll
+      for (int t = 0; t < T; ++t) {
+        const int64_t i = tid + 1024 * t;
+        kk[t] = false;
+        if (i < n_have) {
+#pragma unroll
+          for (int w = 0; w < E; ++w) ke[t][w] = s_cut_dyn[w * kCutActive + i];
+          kk[t] = (int)((word_at(ke[t], q) >> sh) & 255) == (int)bkt;
+        }
+      }
+      __syncthreads();
+#pragma unroll
+      for (int t = 0; t < T; ++t) {
+        if (kk[t]) {
+          const unsigned int qq = atomicAdd(&s_out, 1u);
+#pragma unroll
+          for (int w = 0; w < E; ++w) s_cut_dyn[w * kCutActive + qq] = ke[t][w];
+        }
+      }
+      __syncthreads();
+    }
+    n_act = s_pick[2];
+    if ((int64_t)s_pick[2] == k_rem) {  // the whole bucket is in: every entry with this prefix passes
+      const uint64_t low = sh ? ((1ULL << sh) - 1) : 0;
+#pragma unroll
+      for (int w = 0; w < E; ++w) {
+        if (w == q) th[w] |= low;
+        if (w > q) th[w] = ~0ULL;
+      }
+      closed = true;
+    }
+    __syncthreads();
+  }
+  // compaction of the entries <= threshold into the scratch arrays (at most k of them)
+  if (tid == 0) s_out = 0;
+  __syncthreads();
+  for (int64_t i0 = tid - lane; i0 < n; i0 += 1024) {
+    const int64_t i = i0 + lane;
+    uint64_t e[E];
+    bool keep = false;
+    if (i < n) {
+      load_entry(i, e);
+      keep = img_le(e, th);
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    if (!bal) continue;
+    unsigned int base = 0;
+    if (lane == __ffs(bal) - 1) base = atomicAdd(&s_out, (unsigned)__popc(bal));
+    base = __shfl_sync(0xffffffffu, base, __ffs(bal) - 1);
+    if (keep) {
+      const unsigned int qq = base + __popc(bal & ((1u << lane) - 1));
+      if ((int64_t)qq < a.k) {
+#pragma unroll
+        for (int w = 0; w < W; ++w) a.alt_img[w * a.k + qq] = e[w];
+        a.alt_rowid[qq] = e[W];
+        a.alt_bits[qq] = l.bits[i];
+      }
+    }
+  }
+  __syncthreads();
+  const int64_t kept = (int64_t)s_out < a.k ? (int64_t)s_out : a.k;
+  for (int64_t i = tid; i < kept; i += 1024) {
+#pragma unroll
+    for (int w = 0; w < W; ++w) l.img[w * l.cap + i] = a.alt_img[w * a.k + i];
+    l.rowid[i] = a.alt_rowid[i];
+    l.bits[i] = a.alt_bits[i];
+  }
+  if (tid == 0) {
+    l.state[ST_COUNT] = (unsigned long long)kept;
+#pragma unroll
+    for (int w = 0; w < W; ++w) l.state[MST_BOUND + w] = th[w];
+  }
+}
+
+// n <= 4096 candidates ranked by (image, row id) inside one CTA; out_idx[rank] = entry.
+template <int W>
+__global__ void __launch_bounds__(1024) small_rank_sort_multi_kernel(const uint64_t* img, int64_t stride, const uint64_t* rowid, int n,
+                                                                     uint32_t* out_idx) {
+  constexpr int E = W + 1;
+  extern __shared__ __align__(16) uint64_t s_ent[];  // [E][n]
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+#pragma unroll
+    for (int w = 0; w < W; ++w) s_ent[w * n + i] = img[w * stride + i];
+    s_ent[W * n + i] = rowid[i];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    uint64_t e[E];
+#pragma unroll
+    for (int w = 0; w < E; ++w) e[w] = s_ent[w * n + i];
+    int rank = 0;
+    for (int j = 0; j < n; ++j) {
+      bool lt = false;  // entry j < entry i
+#pragma unroll
+      for (int w = E - 1; w >= 0; --w) {
+        const uint64_t x = s_ent[w * n + j];
+        lt = x < e[w] || (x == e[w] && lt);
+      }
+      rank += lt;
+    }
+    out_idx[rank] = (uint32_t)i;
+  }
+}
+
+// Result block [first key, row id] from the sorted permutation; a row is NULL when its placement
+// bit (the image's top bit) says so.
+struct MultiEmitArgs {
+  const uint32_t* idx;
+  const uint64_t* img0;
+  const uint64_t* rowid;
+  const uint64_t* bits;
+  int64_t n;
+  int32_t dtype, nullable, nulls_first;
+  void* out_key;
+  int64_t* out_row;
+  uint8_t* out_valid_bytes;
+  unsigned long long* n_null;
+};
+__global__ void topk_multi_emit_kernel(const __grid_constant__ MultiEmitArgs a) {
+  unsigned int nulls = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t j = a.idx[i];
+    const bool ok = !a.nullable || (int)(a.img0[j] >> 63) == (a.nulls_first != 0);
+    store_narrow_key(a.out_key, i, a.dtype, ok ? a.bits[j] : 0);
+    a.out_row[i] = (int64_t)a.rowid[j];
+    a.out_valid_bytes[i] = ok ? 1 : 0;
+    nulls += !ok;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) nulls += __shfl_xor_sync(0xffffffffu, nulls, o);
+  if ((threadIdx.x & 31) == 0 && nulls) atomicAdd(a.n_null, (unsigned long long)nulls);
+}
+
 }  // namespace
 
 // ================================================================ operator
@@ -529,6 +983,13 @@ class TopkOp : public Op {
   int x_dtype[DBX_MAX_SORT_KEYS - 1] = {}, x_cls[DBX_MAX_SORT_KEYS - 1] = {};
   bool x_nullable[DBX_MAX_SORT_KEYS - 1] = {};
   DevBuf x_ord[DBX_MAX_SORT_KEYS - 1], x_rid[DBX_MAX_SORT_KEYS - 1], x_cnt, w_ord[2], w_rid[2];
+  // ---- streaming top-k over several keys: one candidate list of composite images (rowid, bits and
+  // alt_rowid, alt_bits as in top-k mode; no NULL list)
+  bool multi = false;
+  int mw = 0;    // image words
+  MultiKeys mk;  // image layout; the columns of the block being pushed
+  DevBuf m_img, m_state, alt_img, snap_img;
+  int scan_multi_ctas_per_sm = 0;
   std::unique_ptr<OwnedBlock> result;
   bool pulled = false;
 
@@ -553,18 +1014,40 @@ class TopkOp : public Op {
       if (dtype_size(x_dtype[j]) == 0) { err.set("sort: keys must be numeric columns"); return DBX_ERR_UNSUPPORTED; }
       x_cls[j] = x_dtype[j] == DBX_U64 ? VC_UINT : (dtype_class(x_dtype[j]) == VC_FLT ? VC_FLT : VC_INT);
     }
-    if (n_extra > 0) full_sort = true;  // several keys: sort everything, LIMIT cuts the sorted result
+    // several keys with a LIMIT: streaming top-k over the composite order image
+    multi = n_extra > 0 && !full_sort;
     DBX_CUDA_TRY(err, x_cnt.ensure(64));
     DBX_TRY(stager.init(dev, stream, &err));
     DBX_CUDA_TRY(err, host.ensure(256));
     DBX_CUDA_TRY(err, state.ensure(8 * ST_WORDS * 3 + 64));
+    if (multi) {
+      int dts[DBX_MAX_SORT_KEYS] = {key_dtype};
+      bool nul[DBX_MAX_SORT_KEYS] = {key_nullable};
+      memset(&mk, 0, sizeof(mk));
+      mk.asc[0] = p->asc; mk.nulls_first[0] = p->nulls_first;
+      for (int j = 0; j < n_extra; ++j) {
+        dts[1 + j] = x_dtype[j]; nul[1 + j] = x_nullable[j];
+        mk.asc[1 + j] = p->extra_asc[j]; mk.nulls_first[1 + j] = p->extra_nulls_first[j];
+      }
+      mw = multi_key_layout(dts, nul, 1 + n_extra, &mk);
+      DBX_CUDA_TRY(err, m_state.ensure(8 * (ST_WORDS + kMaxImageWords)));
+    }
     if (!full_sort) {
       const int64_t k = p->limit;
       // candidate list: large enough that a whole device-resident column usually fits behind the
-      // boundary of its first few million rows; 3 x 8 B per entry
+      // boundary of its first few million rows; 3 x 8 B per entry ((W + 2) x 8 B for W image words)
       static const int64_t cap_env = getenv("DBX_TOPK_CAP") ? atoll(getenv("DBX_TOPK_CAP")) : 0;
       cap = cap_env > 0 ? cap_env : std::max<int64_t>(1 << 22, 8 * k);
       cap = std::max<int64_t>(cap, 4 * k + 4096);
+      if (multi) {
+        DBX_CUDA_TRY(err, m_img.ensure(mw * cap * 8));
+        DBX_CUDA_TRY(err, rowid.ensure(cap * 8));
+        DBX_CUDA_TRY(err, bits.ensure(cap * 8));
+        DBX_CUDA_TRY(err, alt_img.ensure(mw * k * 8));
+        DBX_CUDA_TRY(err, alt_rowid.ensure(k * 8));
+        DBX_CUDA_TRY(err, alt_bits.ensure(k * 8));
+        return reset();
+      }
       DBX_CUDA_TRY(err, ord.ensure(cap * 8));
       DBX_CUDA_TRY(err, rowid.ensure(cap * 8));
       DBX_CUDA_TRY(err, bits.ensure(cap * 8));
@@ -583,6 +1066,10 @@ class TopkOp : public Op {
     topk_reset_kernel<<<1, 32, 0, stream>>>((unsigned long long*)state.p);  // count 0, boundary = everything passes
     count_launch();
     DBX_CUDA_TRY(err, cudaMemsetAsync(x_cnt.p, 0, 64, stream));
+    if (multi) {  // count 0, boundary all ones: everything passes
+      DBX_CUDA_TRY(err, cudaMemsetAsync(m_state.p, 0, 8 * MST_BOUND, stream));
+      DBX_CUDA_TRY(err, cudaMemsetAsync((unsigned long long*)m_state.p + MST_BOUND, 0xFF, 8 * mw, stream));
+    }
     DBX_CUDA_TRY(err, cudaGetLastError());
     count_ub = null_ub = 0;
     rows_seen = 0;
@@ -607,8 +1094,76 @@ class TopkOp : public Op {
     return l;
   }
 
+  MultiList multi_list() const {
+    MultiList l;
+    l.img = (uint64_t*)m_img.p; l.rowid = (uint64_t*)rowid.p; l.bits = (uint64_t*)bits.p;
+    l.state = (unsigned long long*)m_state.p;
+    l.cap = cap;
+    return l;
+  }
+  // calls f(std::integral_constant<int, W>) for this operator's image width
+  template <class F>
+  int32_t by_words(F&& f) {
+    switch (mw) {
+      case 1: return f(std::integral_constant<int, 1>());
+      case 2: return f(std::integral_constant<int, 2>());
+      case 3: return f(std::integral_constant<int, 3>());
+      case 4: return f(std::integral_constant<int, 4>());
+      case 5: return f(std::integral_constant<int, 5>());
+      default: err.set("internal: composite sort image wider than 5 words"); return DBX_ERR_INVALID;
+    }
+  }
+  template <int W>
+  int32_t multi_cut_w(int64_t threshold) {
+    MultiCutArgs a;
+    a.l = multi_list();
+    a.alt_img = (uint64_t*)alt_img.p; a.alt_rowid = (uint64_t*)alt_rowid.p; a.alt_bits = (uint64_t*)alt_bits.p;
+    a.k = prm.limit; a.threshold = threshold;
+    const int smem = kCutActive * (W + 1) * 8;  // 192 KiB at W = 5
+    static std::atomic<bool> attr_set[64];
+    if (!attr_set[device]) {
+      DBX_CUDA_TRY(err, cudaFuncSetAttribute(topk_multi_cut_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+      attr_set[device] = true;
+    }
+    topk_multi_cut_kernel<W><<<1, 1024, smem, stream>>>(a);
+    count_launch();
+    return DBX_OK;
+  }
+  template <int W>
+  int32_t multi_scan_w(const MultiKeys& k, int64_t m, int64_t row_base, bool fast) {
+    if (scan_multi_ctas_per_sm == 0) {
+      int a = 0, b2 = 0;
+      DBX_CUDA_TRY(err, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, topk_multi_scan_kernel<W, true>, 256, 0));
+      DBX_CUDA_TRY(err, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, topk_multi_scan_kernel<W, false>, 256, 0));
+      scan_multi_ctas_per_sm = std::max(1, std::min(a, b2));
+    }
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((m + 2047) / 2048, (int64_t)kNumSMs * scan_multi_ctas_per_sm));
+    if (fast) topk_multi_scan_kernel<W, true><<<grid, 256, 0, stream>>>(k, m, row_base, multi_list());
+    else topk_multi_scan_kernel<W, false><<<grid, 256, 0, stream>>>(k, m, row_base, multi_list());
+    count_launch();
+    return DBX_OK;
+  }
+  int32_t launch_multi_scan(int64_t off, int64_t m, int64_t row_base) {
+    MultiKeys k = mk;
+    for (int c = 0; c < mk.n_keys; ++c) {
+      k.col[c].data = (const char*)mk.col[c].data + off * dtype_size(mk.col[c].dtype);
+      if (k.col[c].validity) k.col[c].vbit_off += off;
+    }
+    const bool fast = !key_nullable && dtype_size(key_dtype) == 8 && !k.col[0].validity && ((reinterpret_cast<uintptr_t>(k.col[0].data) & 31) == 0);
+    DBX_TRY(by_words([&](auto w) { return multi_scan_w<decltype(w)::value>(k, m, row_base, fast); }));
+    DBX_CUDA_TRY(err, cudaGetLastError());
+    return DBX_OK;
+  }
+
   // cut both lists back to k when they hold more than `threshold` entries (device decides)
   int32_t launch_cuts(int64_t threshold, int64_t rows_so_far) {
+    if (multi) {
+      DBX_TRY(by_words([&](auto w) { return multi_cut_w<decltype(w)::value>(threshold); }));
+      DBX_CUDA_TRY(err, cudaGetLastError());
+      count_ub = std::min(count_ub, std::max(threshold, prm.limit));
+      rows_at_last_cut = rows_so_far;
+      return DBX_OK;
+    }
     CutArgs a;
     a.l = cand_list();
     a.alt_ord = (uint64_t*)alt_ord.p; a.alt_rowid = (uint64_t*)alt_rowid.p; a.alt_bits = (uint64_t*)alt_bits.p;
@@ -636,6 +1191,7 @@ class TopkOp : public Op {
   }
 
   int32_t launch_scan(const DevCol& col, int64_t off, int64_t m, int64_t row_base) {
+    if (multi) return launch_multi_scan(off, m, row_base);  // mk.col[] holds the pushed block's keys
     DevCol c = col;
     const int esz = dtype_size(key_dtype);
     c.data = (const char*)col.data + off * esz;
@@ -667,7 +1223,7 @@ class TopkOp : public Op {
       const int64_t piece = std::min(m - done, room);
       DBX_TRY(launch_scan(col, off + done, piece, rows_seen + off + done));
       count_ub += piece;
-      if (key_nullable) null_ub += piece;
+      if (key_nullable && !multi) null_ub += piece;
       done += piece;
     }
     return DBX_OK;
@@ -685,7 +1241,8 @@ class TopkOp : public Op {
     int64_t chunk = std::max<int64_t>(8 * k, 1 << 14);
     bool snap = false;
     int64_t snap_done = 0, snap_count_ub = 0, snap_null_ub = 0, snap_cut_pos = 0;
-    unsigned long long* st = (unsigned long long*)state.p;
+    unsigned long long* st = (unsigned long long*)(multi ? m_state.p : state.p);
+    const size_t st_bytes = multi ? 8 * (MST_BOUND + mw) : 8 * ST_WORDS * 2;  // <= 72 B
     while (done < n) {
       const int64_t seen = rows_seen + done;
       const int64_t rest = n - done;
@@ -697,46 +1254,53 @@ class TopkOp : public Op {
       }
       if (m > room && !snap) {  // first optimistic chunk of this push: snapshot the (cut) lists and their state
         DBX_TRY(launch_cuts(k, seen));
-        DBX_CUDA_TRY(err, snap_ord.ensure(k * 8));
         DBX_CUDA_TRY(err, snap_rowid.ensure(k * 8));
         DBX_CUDA_TRY(err, snap_bits.ensure(k * 8));
-        DBX_CUDA_TRY(err, cudaMemcpyAsync(snap_ord.p, ord.p, k * 8, cudaMemcpyDeviceToDevice, stream));
+        if (multi) {
+          DBX_CUDA_TRY(err, snap_img.ensure(mw * k * 8));
+          DBX_CUDA_TRY(err, cudaMemcpy2DAsync(snap_img.p, k * 8, m_img.p, cap * 8, k * 8, mw, cudaMemcpyDeviceToDevice, stream));
+        } else {
+          DBX_CUDA_TRY(err, snap_ord.ensure(k * 8));
+          DBX_CUDA_TRY(err, cudaMemcpyAsync(snap_ord.p, ord.p, k * 8, cudaMemcpyDeviceToDevice, stream));
+        }
         DBX_CUDA_TRY(err, cudaMemcpyAsync(snap_rowid.p, rowid.p, k * 8, cudaMemcpyDeviceToDevice, stream));
         DBX_CUDA_TRY(err, cudaMemcpyAsync(snap_bits.p, bits.p, k * 8, cudaMemcpyDeviceToDevice, stream));
-        if (key_nullable) {
+        if (key_nullable && !multi) {
           DBX_CUDA_TRY(err, snap_null.ensure(k * 8));
           DBX_CUDA_TRY(err, cudaMemcpyAsync(snap_null.p, null_rowid.p, k * 8, cudaMemcpyDeviceToDevice, stream));
         }
-        DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, st, 8 * ST_WORDS * 2, cudaMemcpyDeviceToHost, stream));
+        DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, st, st_bytes, cudaMemcpyDeviceToHost, stream));
         snap = true;
         snap_done = done; snap_count_ub = count_ub; snap_null_ub = null_ub; snap_cut_pos = rows_at_last_cut;
       }
       DBX_TRY(launch_scan(col, done, m, seen));
       count_ub += m;
-      if (key_nullable) null_ub += m;
+      if (key_nullable && !multi) null_ub += m;
       done += m;
       // cut when the rows seen have doubled since the last cut (always inside a multi-chunk push)
       if (rows_seen + done - rows_at_last_cut >= rows_at_last_cut || done < n) DBX_TRY(launch_cuts(2 * k, rows_seen + done));
       chunk *= 8;
     }
     if (snap) {
-      DBX_CUDA_TRY(err, cudaMemcpyAsync((char*)host.p + 64, st, 8 * ST_WORDS * 2, cudaMemcpyDeviceToHost, stream));
+      DBX_CUDA_TRY(err, cudaMemcpyAsync((char*)host.p + 128, st, st_bytes, cudaMemcpyDeviceToHost, stream));
       DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
       const unsigned long long* before = (const unsigned long long*)host.p;
-      const unsigned long long* after = (const unsigned long long*)((char*)host.p + 64);
-      if (after[ST_OVERFLOW] || after[ST_WORDS + ST_OVERFLOW]) {
+      const unsigned long long* after = (const unsigned long long*)((char*)host.p + 128);
+      if (after[ST_OVERFLOW] || (!multi && after[ST_WORDS + ST_OVERFLOW])) {
         // an optimistic chunk did not fit: back to the snapshot, then the same rows in pieces that do
-        unsigned long long back[2 * ST_WORDS];
-        memcpy(back, before, sizeof(back));
-        back[ST_OVERFLOW] = back[ST_WORDS + ST_OVERFLOW] = 0;
-        DBX_CUDA_TRY(err, cudaMemcpyAsync(ord.p, snap_ord.p, k * 8, cudaMemcpyDeviceToDevice, stream));
+        unsigned long long back[MST_BOUND + kMaxImageWords];
+        memcpy(back, before, st_bytes);
+        back[ST_OVERFLOW] = 0;
+        if (!multi) back[ST_WORDS + ST_OVERFLOW] = 0;
+        if (multi) DBX_CUDA_TRY(err, cudaMemcpy2DAsync(m_img.p, cap * 8, snap_img.p, k * 8, k * 8, mw, cudaMemcpyDeviceToDevice, stream));
+        else DBX_CUDA_TRY(err, cudaMemcpyAsync(ord.p, snap_ord.p, k * 8, cudaMemcpyDeviceToDevice, stream));
         DBX_CUDA_TRY(err, cudaMemcpyAsync(rowid.p, snap_rowid.p, k * 8, cudaMemcpyDeviceToDevice, stream));
         DBX_CUDA_TRY(err, cudaMemcpyAsync(bits.p, snap_bits.p, k * 8, cudaMemcpyDeviceToDevice, stream));
-        if (key_nullable) DBX_CUDA_TRY(err, cudaMemcpyAsync(null_rowid.p, snap_null.p, k * 8, cudaMemcpyDeviceToDevice, stream));
-        DBX_CUDA_TRY(err, cudaMemcpyAsync(st, back, sizeof(back), cudaMemcpyHostToDevice, stream));
+        if (key_nullable && !multi) DBX_CUDA_TRY(err, cudaMemcpyAsync(null_rowid.p, snap_null.p, k * 8, cudaMemcpyDeviceToDevice, stream));
+        DBX_CUDA_TRY(err, cudaMemcpyAsync(st, back, st_bytes, cudaMemcpyHostToDevice, stream));
         DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
         count_ub = std::min<int64_t>(snap_count_ub, (int64_t)before[ST_COUNT]);
-        null_ub = std::min<int64_t>(snap_null_ub, (int64_t)before[ST_WORDS + ST_COUNT]);
+        null_ub = multi ? 0 : std::min<int64_t>(snap_null_ub, (int64_t)before[ST_WORDS + ST_COUNT]);
         rows_at_last_cut = snap_cut_pos;
         DBX_TRY(scan_guaranteed(col, snap_done, n - snap_done));
       }
@@ -796,6 +1360,17 @@ class TopkOp : public Op {
         DBX_CUDA_TRY(err, cudaGetLastError());
       }
     } else {
+      if (multi) {
+        mk.col[0] = col;
+        mk.col[0].dtype = key_dtype;
+        for (int j = 0; j < n_extra; ++j) {
+          const dbx_column& xc = b->cols[prm.extra_key_cols[j]];
+          if (xc.dtype != x_dtype[j] || xc.len != n || xc.is_const) { err.set("push: sort key column does not match the input schema (constant keys unsupported)"); return DBX_ERR_INVALID; }
+          if (xc.validity && !x_nullable[j]) { err.set("push: validity bitmap on a key column declared non-nullable"); return DBX_ERR_INVALID; }
+          DBX_TRY(stager.stage(xc, 1 + j, &mk.col[1 + j]));
+          mk.col[1 + j].dtype = x_dtype[j];
+        }
+      }
       DBX_TRY(push_topk(col, n));
     }
     rows_seen += n;
@@ -934,8 +1509,102 @@ class TopkOp : public Op {
     return DBX_OK;
   }
 
+  // the sorted order of n <= k multi-key candidates as a permutation of the list (`*idx`)
+  template <int W>
+  int32_t multi_order_w(int64_t n, uint32_t** idx) {
+    DBX_CUDA_TRY(err, f_idx0.ensure(std::max<int64_t>(n, 1) * 4));
+    *idx = (uint32_t*)f_idx0.p;
+    if (n == 0) return DBX_OK;
+    const uint64_t* img = (const uint64_t*)m_img.p;
+    if (n <= 4096) {
+      static std::atomic<bool> attr_set[64];
+      if (!attr_set[device]) {
+        DBX_CUDA_TRY(err, cudaFuncSetAttribute(small_rank_sort_multi_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * (W + 1) * 8));
+        attr_set[device] = true;
+      }
+      small_rank_sort_multi_kernel<W><<<1, 1024, (size_t)n * (W + 1) * 8, stream>>>(img, cap, (const uint64_t*)rowid.p, (int)n, *idx);
+      count_launch();
+      DBX_CUDA_TRY(err, cudaGetLastError());
+      return DBX_OK;
+    }
+    // W + 1 stable radix sorts of a permutation: by row id, then by the image words from the least
+    // significant to the most significant
+    DBX_CUDA_TRY(err, f_idx1.ensure(n * 4));
+    DBX_CUDA_TRY(err, f_key0.ensure(n * 8));
+    DBX_CUDA_TRY(err, f_key1.ensure(n * 8));
+    uint32_t* cur = (uint32_t*)f_idx0.p;
+    uint32_t* other = (uint32_t*)f_idx1.p;
+    iota_u32_kernel<<<grid_1d(n), 256, 0, stream>>>(cur, n);
+    count_launch();
+    DBX_CUDA_TRY(err, cudaMemcpyAsync(f_key0.p, rowid.p, n * 8, cudaMemcpyDeviceToDevice, stream));
+    int rid_bits = 8;
+    while (rid_bits < 64 && ((uint64_t)std::max<int64_t>(rows_seen - 1, 0) >> rid_bits)) rid_bits += 8;
+    for (int w = W; w >= 0; --w) {
+      if (w < W) {
+        gather_u64_kernel<<<grid_1d(n), 256, 0, stream>>>(img + (size_t)w * cap, cur, (uint64_t*)f_key0.p, n);
+        count_launch();
+      }
+      int buf = 0;
+      DBX_TRY(sorter.sort(err, stream, (uint64_t*)f_key0.p, (uint64_t*)f_key1.p, cur, other, n, 0, w == W ? rid_bits : 64, false, 0, 0, &buf));
+      if (buf) std::swap(cur, other);
+    }
+    *idx = cur;
+    DBX_CUDA_TRY(err, cudaGetLastError());
+    return DBX_OK;
+  }
+
+  int32_t finish_multi() {
+    const int64_t k = prm.limit;
+    DBX_TRY(launch_cuts(k, rows_seen));  // the list down to <= k entries
+    DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, m_state.p, 8 * ST_WORDS, cudaMemcpyDeviceToHost, stream));
+    DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
+    const unsigned long long* h = (const unsigned long long*)host.p;
+    if (h[ST_OVERFLOW]) { err.set("internal: top-k candidate list overflow"); return DBX_ERR_CUDA; }
+    const int64_t n_out = std::min<int64_t>((int64_t)h[ST_COUNT], k);
+    uint32_t* idx = nullptr;
+    DBX_TRY(by_words([&](auto w) { return multi_order_w<decltype(w)::value>(n_out, &idx); }));
+    auto ob = std::make_unique<OwnedBlock>();
+    ob->stream = stream;  // freed in order behind this operator's enqueued work
+    ob->device = device;
+    const int esz = dtype_size(key_dtype);
+    void *okey = nullptr, *orow = nullptr, *ovb = nullptr, *obits = nullptr;
+    DBX_TRY(dev_alloc(ob.get(), (size_t)n_out * esz, &okey));
+    DBX_TRY(dev_alloc(ob.get(), (size_t)n_out * 8, &orow));
+    DBX_TRY(dev_alloc(ob.get(), (size_t)n_out + 1, &ovb));
+    DBX_TRY(dev_alloc(ob.get(), (size_t)(n_out + 7) / 8 + 8, &obits));
+    if (n_out) {
+      MultiEmitArgs ea;
+      ea.idx = idx; ea.img0 = (const uint64_t*)m_img.p; ea.rowid = (const uint64_t*)rowid.p; ea.bits = (const uint64_t*)bits.p;
+      ea.n = n_out; ea.dtype = key_dtype; ea.nullable = key_nullable; ea.nulls_first = prm.nulls_first;
+      ea.out_key = okey; ea.out_row = (int64_t*)orow; ea.out_valid_bytes = (uint8_t*)ovb;
+      ea.n_null = (unsigned long long*)m_state.p + MST_NULLS;
+      topk_multi_emit_kernel<<<grid_1d(n_out), 256, 0, stream>>>(ea);
+      pack_bits_kernel<<<grid_1d((n_out + 7) / 8), 256, 0, stream>>>((const uint8_t*)ovb, n_out, (uint8_t*)obits);
+      count_launch(2);
+      DBX_CUDA_TRY(err, cudaGetLastError());
+    }
+    const bool radix = n_out > 4096 && sorter.meta.p;
+    DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, (unsigned long long*)m_state.p + MST_NULLS, 8, cudaMemcpyDeviceToHost, stream));
+    if (radix) DBX_CUDA_TRY(err, cudaMemcpyAsync((char*)host.p + 8, (void*)sorter.fail(), 4, cudaMemcpyDeviceToHost, stream));
+    DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
+    const int64_t n_nulls = (int64_t)*(const unsigned long long*)host.p;
+    if (radix && *(const unsigned int*)((char*)host.p + 8)) { err.set("internal: radix sort look-back timed out"); return DBX_ERR_CUDA; }
+    dbx_column kcol;
+    memset(&kcol, 0, sizeof(kcol));
+    kcol.dtype = key_dtype; kcol.mem = DBX_MEM_DEVICE; kcol.len = n_out; kcol.data = okey;
+    if (key_nullable) { kcol.validity = (const uint8_t*)obits; kcol.null_count = n_nulls; }
+    dbx_column rcol;
+    memset(&rcol, 0, sizeof(rcol));
+    rcol.dtype = DBX_I64; rcol.mem = DBX_MEM_DEVICE; rcol.len = n_out; rcol.data = orow;
+    ob->cols.push_back(kcol);
+    ob->cols.push_back(rcol);
+    result = std::move(ob);
+    return DBX_OK;
+  }
+
   int32_t finish() override {
     if (full_sort) return finish_full_sort();
+    if (multi) return finish_multi();
     const int64_t k = prm.limit;
     DBX_TRY(launch_cuts(k, rows_seen));  // both lists down to <= k entries
     unsigned long long* st = (unsigned long long*)state.p;

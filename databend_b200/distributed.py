@@ -95,47 +95,69 @@ def partitioned_hash_join(build: DataBlock, probe: DataBlock, build_key, probe_k
     return out, j, (keep_b, keep_p)
 
 
+def _pack_i64(vals: np.ndarray) -> np.ndarray:
+    if vals.dtype.itemsize == 8:
+        return np.ascontiguousarray(vals).view(np.int64)
+    return vals.astype(np.float64).view(np.int64) if vals.dtype.kind == "f" else vals.astype(np.int64)
+
+
+def _unpack_i64(raw: np.ndarray, dtype: np.dtype) -> np.ndarray:
+    if dtype.itemsize == 8:
+        return raw.view(dtype)
+    return raw.view(np.float64).astype(dtype) if dtype.kind == "f" else raw.astype(dtype)
+
+
 def topk_merge(local: DataBlock, row_base: int, k: int, asc: bool, nulls_first: bool, device: int = 0, group=None,
-               final_op: TransformTopN = None) -> DataBlock:
+               final_op: TransformTopN = None, extra_keys: Sequence[Tuple[Column, bool, bool]] = ()) -> DataBlock:
     """All-gather every rank's top-k block ([key, row id], already in output order) and run the
     final TransformTopN over the gathered candidates.  Candidates are concatenated in rank order,
-    so equal keys keep ascending GLOBAL row ids (rank r's rows precede rank r+1's)."""
+    so equal keys keep ascending GLOBAL row ids (rank r's rows precede rank r+1's).
+
+    extra_keys: the later keys of ORDER BY a, b, ... as (column, asc, nulls_first), each column
+    holding the rank's candidate values in the block's row order (taken by row id from the local
+    input, e.g. with kernels.take).  The final TransformTopN then breaks ties on them, so equal
+    composite keys keep ascending global row ids.  A caller-supplied final_op must be built with
+    the same extra keys at offsets 1, 2, ...."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     keys = local.columns[0]
-    vals_l, valid_l = keys.values(), keys.valid_mask()
+    cols_l = [keys] + [c for c, _, _ in extra_keys]
+    vals_l = [c.values() for c in cols_l]
+    valid_l = [c.valid_mask() for c in cols_l]
     rows_l = local.columns[1].values().astype(np.int64) + row_base
+    nk = len(cols_l)
     if world > 1:
-        # fixed-size tensors (k slots per rank, count in front): one all_gather, no pickling
-        n = len(vals_l)
+        # fixed-size tensors (k slots per rank and per array, count in front): one all_gather, no pickling
+        n = len(rows_l)
+        width = 1 + (2 * nk + 1) * k
         dev = torch.device("cuda", device) if dist.get_backend(group) == "nccl" else torch.device("cpu")
-        buf = torch.zeros(1 + 3 * k, dtype=torch.int64, device=dev)
-        pack = np.zeros(1 + 3 * k, dtype=np.int64)
+        buf = torch.zeros(width, dtype=torch.int64, device=dev)
+        pack = np.zeros(width, dtype=np.int64)
         pack[0] = n
-        pack[1:1 + n] = np.ascontiguousarray(vals_l).view(np.int64) if vals_l.dtype.itemsize == 8 else vals_l.astype(np.float64).view(np.int64) if vals_l.dtype.kind == "f" else vals_l.astype(np.int64)
-        pack[1 + k:1 + k + n] = valid_l.astype(np.int64)
-        pack[1 + 2 * k:1 + 2 * k + n] = rows_l
+        for j in range(nk):
+            pack[1 + 2 * j * k:1 + 2 * j * k + n] = _pack_i64(vals_l[j])
+            pack[1 + (2 * j + 1) * k:1 + (2 * j + 1) * k + n] = valid_l[j].astype(np.int64)
+        pack[1 + 2 * nk * k:1 + 2 * nk * k + n] = rows_l
         buf.copy_(torch.from_numpy(pack))
-        out = torch.empty(world * (1 + 3 * k), dtype=torch.int64, device=dev)
+        out = torch.empty(world * width, dtype=torch.int64, device=dev)
         dist.all_gather_into_tensor(out, buf, group=group)
-        g = out.cpu().numpy().reshape(world, 1 + 3 * k)
-        vs, ms, rs = [], [], []
+        g = out.cpu().numpy().reshape(world, width)
+        vs, ms, rs = [[] for _ in range(nk)], [[] for _ in range(nk)], []
         for r in range(world):
             m = int(g[r, 0])
-            raw = g[r, 1:1 + m]
-            if vals_l.dtype.itemsize == 8:
-                vs.append(raw.view(vals_l.dtype))
-            elif vals_l.dtype.kind == "f":
-                vs.append(raw.view(np.float64).astype(vals_l.dtype))
-            else:
-                vs.append(raw.astype(vals_l.dtype))
-            ms.append(g[r, 1 + k:1 + k + m].astype(bool))
-            rs.append(g[r, 1 + 2 * k:1 + 2 * k + m])
-        vals, valid, rows = np.concatenate(vs), np.concatenate(ms), np.concatenate(rs)
+            for j in range(nk):
+                vs[j].append(_unpack_i64(g[r, 1 + 2 * j * k:1 + 2 * j * k + m], vals_l[j].dtype))
+                ms[j].append(g[r, 1 + (2 * j + 1) * k:1 + (2 * j + 1) * k + m].astype(bool))
+            rs.append(g[r, 1 + 2 * nk * k:1 + 2 * nk * k + m])
+        vals, valid, rows = [np.concatenate(v) for v in vs], [np.concatenate(m) for m in ms], np.concatenate(rs)
     else:
         vals, valid, rows = vals_l, valid_l, rows_l
-    nullable = keys.validity is not None or not valid.all()
-    cand = DataBlock([Column.from_data(vals, keys.dtype, validity=valid if nullable else None)], len(vals))
-    op = final_op or TransformTopN(0, asc, nulls_first, k, schema_types(cand) if nullable else [keys.dtype], device)
+    cand_cols = []
+    for j, c in enumerate(cols_l):
+        nullable = c.validity is not None or not valid[j].all()
+        cand_cols.append(Column.from_data(vals[j], c.dtype, validity=valid[j] if nullable else None))
+    cand = DataBlock(cand_cols, len(rows))
+    op = final_op or TransformTopN(0, asc, nulls_first, k, schema_types(cand), device,
+                                   extra_keys=[(1 + j, a, nf) for j, (_, a, nf) in enumerate(extra_keys)])
     if final_op is not None:
         op.reset()
     op.transform(cand)

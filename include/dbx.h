@@ -196,9 +196,12 @@ typedef struct dbx_topk_params {
   int64_t limit;
   /* ORDER BY key_col, extra_key_cols[0], extra_key_cols[1], ... (SortColumnDescription list,
    * kernels/sort.rs:43-60): ties on the earlier keys are broken by the later ones, each with its own
-   * direction and NULL placement, and finally by input order.  With extra keys the whole input is
-   * sorted on the device (one stable radix sort per key, least significant first) and `limit` > 0
-   * cuts the sorted result.  Result block: [key (first key), row_id Int64] as for one key. */
+   * direction and NULL placement, and finally by input order.  With extra keys and
+   * 1 <= limit <= 4 Mi the streaming top-k runs on a composite order image (per key a NULL-placement
+   * bit if nullable, then the order-preserving value at its natural width; at most 5 x 64 bits),
+   * with no row limit; with limit = 0 or limit > 4 Mi the whole input is sorted on the device (one
+   * stable radix sort per key, least significant first, up to 2^30 - 1 rows) and `limit` > 0 cuts
+   * the sorted result.  Result block: [key (first key), row_id Int64] as for one key. */
   int32_t n_extra_keys; /* 0 .. DBX_MAX_SORT_KEYS - 1 */
   int32_t extra_key_cols[DBX_MAX_SORT_KEYS - 1];
   int32_t extra_asc[DBX_MAX_SORT_KEYS - 1];

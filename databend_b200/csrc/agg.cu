@@ -708,6 +708,13 @@ static size_t partition_smem_for(int ns) {
     case 7: return partition_smem_bytes<7>(); default: return partition_smem_bytes<8>();
   }
 }
+static size_t ring_smem_for(int ns) {
+  switch (ns) {
+    case 1: return ring_smem_bytes<1>(); case 2: return ring_smem_bytes<2>(); case 3: return ring_smem_bytes<3>();
+    case 4: return ring_smem_bytes<4>(); case 5: return ring_smem_bytes<5>(); case 6: return ring_smem_bytes<6>();
+    case 7: return ring_smem_bytes<7>(); default: return ring_smem_bytes<8>();
+  }
+}
 static size_t slice_stage_bytes_for(int ns) {
   switch (ns) {
     case 1: return slice_stage_bytes<1>(); case 2: return slice_stage_bytes<2>(); case 3: return slice_stage_bytes<3>();
@@ -774,7 +781,8 @@ class AggPartialOp : public Op {
                       std::to_string(slice_chunks) + ", in L2 regions: " + std::to_string(partitioned_chunks - slice_chunks) +
                       "), one-pass fallbacks (skew): " + std::to_string(partition_fallbacks) + "; specialised launches: pass 1 " +
                       std::to_string(part_jit_launches) + " of " + std::to_string(partitioned_chunks + partition_fallbacks) + ", pass 2 " +
-                      std::to_string(slice_jit_launches) + " of " + std::to_string(slice_chunks);
+                      std::to_string(slice_jit_launches) + " of " + std::to_string(slice_chunks) + "; pass 1 on the bulk-copy ring: " +
+                      std::to_string(part_ring_launches) + " of " + std::to_string(partitioned_chunks + partition_fallbacks);
     return variant_text.c_str();
   }
   // Ask for kernels compiled for this plan (grouped plans without TMA pairs).  Failure is not an
@@ -815,13 +823,15 @@ class AggPartialOp : public Op {
     // the two passes of the partitioned path: both use more than 48 KB of dynamic shared memory
     ce = cudaKernelSetAttributeForDevice(jit.part, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)partition_smem_for(plan.n_slots), device);
     if (ce == cudaSuccess)
+      ce = cudaKernelSetAttributeForDevice(jit.part_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring_smem_for(plan.n_slots), device);
+    if (ce == cudaSuccess)
       ce = cudaKernelSetAttributeForDevice(jit.slice, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSliceBytes + slice_stage_bytes_for(plan.n_slots)), device);
     if (ce != cudaSuccess) drop_two_pass_jit("shared-memory opt-in", ce);
   }
   // the partitioned passes go back to the precompiled kernels; the fused kernels stay specialised
   void drop_two_pass_jit(const char* what, cudaError_t ce) {
     cudaGetLastError();
-    jit.part = jit.slice = nullptr;
+    jit.part = jit.part_ring = jit.slice = nullptr;
     jit_status += std::string(" (two-pass: precompiled kernels, ") + what + " of the specialised kernel failed: " + cudaGetErrorString(ce) + ")";
   }
 
@@ -1286,11 +1296,40 @@ class AggPartialOp : public Op {
     cudaGetLastError();
   }
   int jit_part_per_sm = 0;  // resident CTAs per SM of the specialised pass 1, 0: not asked yet
-  int64_t part_jit_launches = 0, slice_jit_launches = 0;
+  int jit_ring_per_sm = -1; // the same for its ring variant, -1: not asked yet
+  int64_t part_jit_launches = 0, slice_jit_launches = 0, part_ring_launches = 0;
+  // DBX_AGG_PART_RING=0: pass 1 never takes the bulk-copy ring (both variants can then be compared in one process)
+  bool part_ring = !(getenv("DBX_AGG_PART_RING") && atoi(getenv("DBX_AGG_PART_RING")) == 0);
+  // The ring variant of pass 1 copies whole tiles of every column slot with the bulk-copy unit: it needs
+  // byte-sized integer or float columns that start 16-byte aligned (a tile is then a multiple of 16 bytes).
+  bool ring_fits(const AggKernelParams& kp) const {
+    if (!part_ring) return false;
+    for (int s = 0; s < plan.n_slots; ++s) {
+      const DevCol& c = kp.cols[s];
+      if (c.is_const) continue;
+      if (dtype_size(c.dtype) == 0 || ((uintptr_t)c.data & 15)) return false;
+    }
+    return true;
+  }
   template <int NS>
   int32_t launch_partition(const AggKernelParams& kp, const PartitionOut& po) {
-    const size_t smem = partition_smem_bytes<NS>();
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
+    const int64_t n_tiles = (kp.n_rows + kTileRows - 1) / kTileRows;
+    const bool ring = ring_fits(kp);
+    if (jit.two_pass_ok() && ring && jit_ring_per_sm < 0) {
+      int n = 0;
+      const cudaError_t ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, (const void*)jit.part_ring, kRingThreads, ring_smem_bytes<NS>());
+      if (ce == cudaSuccess) jit_ring_per_sm = n;
+      else drop_two_pass_jit("occupancy query", ce);
+    }
+    if (jit.two_pass_ok() && ring && jit_ring_per_sm > 0) {  // one persistent CTA per SM
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)kNumSMs * jit_ring_per_sm));
+      void* args[] = {(void*)&kp, (void*)&po};
+      const cudaError_t ce = cudaLaunchKernel((const void*)jit.part_ring, dim3(grid), dim3(kRingThreads), args, ring_smem_bytes<NS>(), stream);
+      if (ce == cudaSuccess) { ++part_jit_launches; ++part_ring_launches; return DBX_OK; }
+      drop_two_pass_jit("launch", ce);
+    }
+    const size_t smem = partition_smem_bytes<NS>();
     if (jit.two_pass_ok() && !jit_part_per_sm) {  // the occupancy of the kernel that will run
       int n = 0;
       const cudaError_t ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, (const void*)jit.part, kBlock, smem);
@@ -1298,14 +1337,14 @@ class AggPartialOp : public Op {
       else drop_two_pass_jit("occupancy query", ce);
     }
     if (jit.two_pass_ok()) {
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * jit_part_per_sm));
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)kNumSMs * jit_part_per_sm));
       void* args[] = {(void*)&kp, (void*)&po};
       const cudaError_t ce = cudaLaunchKernel((const void*)jit.part, dim3(grid), dim3(kBlock), args, smem, stream);
       if (ce == cudaSuccess) { ++part_jit_launches; return DBX_OK; }
       drop_two_pass_jit("launch", ce);
     }
-    if (kp.n_comp > 0) return launch_partition_kernel<NS, true>(kp, po);
-    return launch_partition_kernel<NS, false>(kp, po);
+    if (kp.n_comp > 0) return ring ? launch_partition_ring_kernel<NS, true>(kp, po) : launch_partition_kernel<NS, true>(kp, po);
+    return ring ? launch_partition_ring_kernel<NS, false>(kp, po) : launch_partition_kernel<NS, false>(kp, po);
   }
   template <int NS, bool EXPR>
   int32_t launch_partition_kernel(const AggKernelParams& kp, const PartitionOut& po) {
@@ -1320,6 +1359,23 @@ class AggPartialOp : public Op {
     // one resident wave: a CTA copies its survivors out only every few tiles, more CTAs would only add partial batches
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * per_sm[device]));
     filter_partition_kernel<NS, EXPR><<<grid, kBlock, smem, stream>>>(kp, po);
+    return DBX_OK;
+  }
+  template <int NS, bool EXPR>
+  int32_t launch_partition_ring_kernel(const AggKernelParams& kp, const PartitionOut& po) {
+    static std::atomic<int> per_sm[64];  // resident CTAs per SM, -1: the kernel does not fit, 0: not asked yet
+    const size_t smem = ring_smem_bytes<NS>();
+    if (!per_sm[device]) {
+      cudaFuncSetAttribute(filter_partition_ring_kernel<NS, EXPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      int n = 0;
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, filter_partition_ring_kernel<NS, EXPR>, kRingThreads, smem);
+      cudaGetLastError();
+      per_sm[device] = n > 0 ? n : -1;
+    }
+    if (per_sm[device] < 0) return launch_partition_kernel<NS, EXPR>(kp, po);
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * per_sm[device]));
+    filter_partition_ring_kernel<NS, EXPR><<<grid, kRingThreads, smem, stream>>>(kp, po);
+    ++part_ring_launches;
     return DBX_OK;
   }
   template <int NS>

@@ -19,9 +19,10 @@ struct AggJitKernels {
   cudaKernel_t fast = nullptr;  // whole tiles of plain 8-byte columns (FAST)
   cudaKernel_t gen = nullptr;   // any column layout, direct row order
   cudaKernel_t part = nullptr;  // pass 1 of the partitioned aggregation (filter_partition_body)
+  cudaKernel_t part_ring = nullptr;  // the same on the bulk-copy ring (filter_partition_ring_body)
   cudaKernel_t slice = nullptr; // pass 2 in shared memory (slice_agg_body)
   bool ok() const { return fast && gen; }
-  bool two_pass_ok() const { return part && slice; }
+  bool two_pass_ok() const { return part && part_ring && slice; }
 };
 
 // Text of the StaticPlan initialiser for a plan; empty when the plan cannot be specialised.

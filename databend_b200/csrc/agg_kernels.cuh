@@ -865,8 +865,18 @@ __device__ __forceinline__ uint64_t plain_row_key(const AggKernelParams& p, cons
   return key;
 }
 
-// exclusive prefix sum of cnt[0, n) into off[0, n), n <= 4 * kBlock; ends with the block synchronised
+// Barrier `BAR` over the kBlock threads 0 .. kBlock - 1: barrier 0 is __syncthreads; the ring variant of pass 1
+// synchronises its consumer threads on barrier 1, which its producer warp never joins.
+template <int BAR>
+__device__ __forceinline__ void block_sync() {
+  if (BAR == 0) __syncthreads();
+  else asm volatile("bar.sync %0, %1;" ::"n"(BAR), "n"(kBlock) : "memory");
+}
+
+// exclusive prefix sum of cnt[0, n) into off[0, n) by threads 0 .. kBlock - 1, n <= 4 * kBlock; ends with
+// those threads synchronised on barrier BAR
 static_assert(kMaxPartitions <= 4 * kBlock, "block_exclusive_scan: four counts per thread");
+template <int BAR = 0>
 __device__ __forceinline__ void block_exclusive_scan(const unsigned int* cnt, unsigned int* off, int n) {
   __shared__ unsigned int s_warp[kWarpsPerBlock];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -885,7 +895,7 @@ __device__ __forceinline__ void block_exclusive_scan(const unsigned int* cnt, un
     if (lane >= o) inc += v;
   }
   if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
+  block_sync<BAR>();
   unsigned int ex = inc - sum;
   for (int w = 0; w < warp; ++w) ex += s_warp[w];
 #pragma unroll
@@ -894,7 +904,89 @@ __device__ __forceinline__ void block_exclusive_scan(const unsigned int* cnt, un
     if (q < per && i < n) off[i] = ex;
     ex += loc[q];
   }
-  __syncthreads();
+  block_sync<BAR>();
+}
+
+// Filters the thread's rows of one tile (vals / vmask: the tile's slot values, loaded by the caller), tags each
+// survivor with its partition and its rank inside the partition, and appends the survivors to the stash:
+// warps in order, rows of a warp in ballot order.  Threads 0 .. kBlock - 1 take part, synchronised on barrier BAR.
+template <int NS, bool EXPR, int R, int BAR>
+__device__ __forceinline__ void partition_stash_tile(const AggKernelParams& p, const PartitionOut& po, RowVals (&vals)[NS], uint32_t (&vmask)[NS],
+                                                     int64_t tile_base, uint64_t* stash, uint32_t* tag, unsigned int* s_cnt,
+                                                     unsigned int (&s_wcnt)[2][kWarpsPerBlock], int& n_stash, int& parity) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t lt_mask = (1u << lane) - 1;
+  const int64_t r0 = tile_base + (int64_t)kRowsPerThread * threadIdx.x;
+  uint32_t in_range = 0;
+#pragma unroll
+  for (int j = 0; j < kRowsPerThread; ++j)
+    if (r0 + j < p.n_rows) in_range |= 1u << j;
+  // computed values are stashed with the inputs: pass 2 reads them and evaluates nothing
+  if (PLN_COMP(EXPR)) eval_computed<NS, false>(p, 0, PLN(comp_pred), vals, vmask, 0, r0);
+  const uint32_t sel = eval_predicate<NS>(p, vals, vmask, in_range);
+  if (PLN_COMP(EXPR)) eval_computed<NS, false>(p, PLN(comp_pred), PLN(n_comp), vals, vmask, sel, r0);
+  uint32_t tg[kRowsPerThread], bal[kRowsPerThread];
+  int warp_n = 0;
+#pragma unroll
+  for (int j = 0; j < kRowsPerThread; ++j) {
+    tg[j] = 0;
+    if ((sel >> j) & 1) {
+      const uint64_t key = plain_row_key<NS>(p, vals, j);
+      const int part = key == kEmptyKey ? 0 : (int)((agg_hash_u64(key) & po.nb_mask) >> po.region_shift);
+      tg[j] = ((uint32_t)part << 16) | atomicAdd(&s_cnt[part], 1u);
+    }
+    bal[j] = __ballot_sync(0xffffffffu, (sel >> j) & 1);
+    warp_n += __popc(bal[j]);
+  }
+  // s_wcnt alternates between two buffers, so a warp that runs ahead into the next tile never overwrites
+  // counts still being read
+  if (lane == 0) s_wcnt[parity][warp] = warp_n;
+  block_sync<BAR>();
+  int pos = n_stash, total = 0;
+  for (int w = 0; w < kWarpsPerBlock; ++w) {
+    const int c = s_wcnt[parity][w];
+    if (w < warp) pos += c;
+    total += c;
+  }
+  parity ^= 1;
+#pragma unroll
+  for (int j = 0; j < kRowsPerThread; ++j) {
+    if ((sel >> j) & 1) {
+      const int i = pos + __popc(bal[j] & lt_mask);
+#pragma unroll
+      for (int s = 0; s < NS; ++s) stash[(size_t)s * R + i] = vals[s].v[j];
+      tag[i] = tg[j];
+    }
+    pos += __popc(bal[j]);
+  }
+  n_stash += total;
+}
+
+// Copies the n_stash collected survivors out in partition order: one global reservation per non-empty
+// partition, then consecutive threads store consecutive rows of a run.  Empties the stash and the counts.
+template <int NS, int R, int BAR>
+__device__ __forceinline__ void partition_copy_out(const PartitionOut& po, const uint64_t* stash, const uint32_t* tag, uint16_t* perm,
+                                                   unsigned int* s_cnt, unsigned int* s_off, unsigned long long* s_base, int& n_stash) {
+  block_sync<BAR>();
+  block_exclusive_scan<BAR>(s_cnt, s_off, po.n_parts);
+  for (int r = threadIdx.x; r < po.n_parts; r += kBlock) {
+    const unsigned int c = s_cnt[r];
+    s_base[r] = c ? atomicAdd(&po.counts[r], (unsigned long long)c) : 0ULL;
+  }
+  for (int i = threadIdx.x; i < n_stash; i += kBlock) perm[s_off[tag[i] >> 16] + (tag[i] & 0xFFFF)] = (uint16_t)i;
+  block_sync<BAR>();
+  for (int li = threadIdx.x; li < n_stash; li += kBlock) {
+    const int i = perm[li];
+    const uint32_t part = tag[i] >> 16;
+    const unsigned long long at = s_base[part] + (tag[i] & 0xFFFF);
+    if (at >= (unsigned long long)po.cap_p) { po.counts[po.n_parts] = 1; continue; }  // the host falls back to the one-pass path
+    const unsigned long long d = (unsigned long long)part * (unsigned long long)po.cap_p + at;
+#pragma unroll
+    for (int s = 0; s < NS; ++s) po.out[s][d] = stash[(size_t)s * R + i];
+  }
+  for (int r = threadIdx.x; r < po.n_parts; r += kBlock) s_cnt[r] = 0;
+  n_stash = 0;
+  block_sync<BAR>();  // shared buffers are reused by the next tiles
 }
 
 template <int NS, bool EXPR = false>
@@ -909,8 +1001,6 @@ __device__ __forceinline__ void filter_partition_body(const AggKernelParams& p, 
   __shared__ unsigned int s_off[kMaxPartitions];
   __shared__ unsigned long long s_base[kMaxPartitions];
   __shared__ unsigned int s_wcnt[2][kWarpsPerBlock];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t lt_mask = (1u << lane) - 1;
   const int64_t n_tiles = (p.n_rows + kTileRows - 1) / kTileRows;
   const uint64_t pol = make_policy_evict_first();
   for (int r = threadIdx.x; r < po.n_parts; r += kBlock) s_cnt[r] = 0;
@@ -925,51 +1015,7 @@ __device__ __forceinline__ void filter_partition_body(const AggKernelParams& p, 
     for (int s = 0; s < NS; ++s) load_slot<false>(p.cols[s], tile * kTileRows, p.n_rows, nullptr, pol, vals[s], vmask[s]);
   }
   for (; tile < n_tiles; tile += gridDim.x) {
-    const int64_t tile_base = tile * kTileRows;
-    const int64_t r0 = tile_base + (int64_t)kRowsPerThread * threadIdx.x;
-    uint32_t in_range = 0;
-#pragma unroll
-    for (int j = 0; j < kRowsPerThread; ++j)
-      if (r0 + j < p.n_rows) in_range |= 1u << j;
-    // computed values are stashed with the inputs: pass 2 reads them and evaluates nothing
-    if (PLN_COMP(EXPR)) eval_computed<NS, false>(p, 0, PLN(comp_pred), vals, vmask, 0, r0);
-    const uint32_t sel = eval_predicate<NS>(p, vals, vmask, in_range);
-    if (PLN_COMP(EXPR)) eval_computed<NS, false>(p, PLN(comp_pred), PLN(n_comp), vals, vmask, sel, r0);
-    uint32_t tg[kRowsPerThread], bal[kRowsPerThread];
-    int warp_n = 0;
-#pragma unroll
-    for (int j = 0; j < kRowsPerThread; ++j) {
-      tg[j] = 0;
-      if ((sel >> j) & 1) {
-        const uint64_t key = plain_row_key<NS>(p, vals, j);
-        const int part = key == kEmptyKey ? 0 : (int)((agg_hash_u64(key) & po.nb_mask) >> po.region_shift);
-        tg[j] = ((uint32_t)part << 16) | atomicAdd(&s_cnt[part], 1u);
-      }
-      bal[j] = __ballot_sync(0xffffffffu, (sel >> j) & 1);
-      warp_n += __popc(bal[j]);
-    }
-    // stash positions: warps in order, rows of a warp in ballot order (s_wcnt alternates between two
-    // buffers, so a warp that runs ahead into the next tile never overwrites counts still being read)
-    if (lane == 0) s_wcnt[parity][warp] = warp_n;
-    __syncthreads();
-    int pos = n_stash, total = 0;
-    for (int w = 0; w < kWarpsPerBlock; ++w) {
-      const int c = s_wcnt[parity][w];
-      if (w < warp) pos += c;
-      total += c;
-    }
-    parity ^= 1;
-#pragma unroll
-    for (int j = 0; j < kRowsPerThread; ++j) {
-      if ((sel >> j) & 1) {
-        const int i = pos + __popc(bal[j] & lt_mask);
-#pragma unroll
-        for (int s = 0; s < NS; ++s) stash[(size_t)s * R + i] = vals[s].v[j];
-        tag[i] = tg[j];
-      }
-      pos += __popc(bal[j]);
-    }
-    n_stash += total;
+    partition_stash_tile<NS, EXPR, R, 0>(p, po, vals, vmask, tile * kTileRows, stash, tag, s_cnt, s_wcnt, n_stash, parity);
     // the next tile's loads fly while this one is stashed and copied out
     const int64_t next = tile + gridDim.x;
     if (next < n_tiles) {
@@ -977,27 +1023,140 @@ __device__ __forceinline__ void filter_partition_body(const AggKernelParams& p, 
       for (int s = 0; s < NS; ++s) load_slot<false>(p.cols[s], next * kTileRows, p.n_rows, nullptr, pol, vals[s], vmask[s]);
     }
     if (n_stash + kTileRows <= R && next < n_tiles) continue;
-    // ---- copy out the collected survivors
-    __syncthreads();
-    block_exclusive_scan(s_cnt, s_off, po.n_parts);
-    for (int r = threadIdx.x; r < po.n_parts; r += kBlock) {
-      const unsigned int c = s_cnt[r];
-      s_base[r] = c ? atomicAdd(&po.counts[r], (unsigned long long)c) : 0ULL;
-    }
-    for (int i = threadIdx.x; i < n_stash; i += kBlock) perm[s_off[tag[i] >> 16] + (tag[i] & 0xFFFF)] = (uint16_t)i;
-    __syncthreads();
-    for (int li = threadIdx.x; li < n_stash; li += kBlock) {
-      const int i = perm[li];
-      const uint32_t part = tag[i] >> 16;
-      const unsigned long long at = s_base[part] + (tag[i] & 0xFFFF);
-      if (at >= (unsigned long long)po.cap_p) { po.counts[po.n_parts] = 1; continue; }  // the host falls back to the one-pass path
-      const unsigned long long d = (unsigned long long)part * (unsigned long long)po.cap_p + at;
+    partition_copy_out<NS, R, 0>(po, stash, tag, perm, s_cnt, s_off, s_base, n_stash);
+  }
+}
+
+// ---------------------------------------------------------------- pass 1, bulk-copy ring variant
+// Same filter, tags, stash and copy-out as filter_partition_body, with the column reads taken off the
+// threads that filter.  One persistent CTA per SM: warps 0-7 (kBlock threads, barrier 1) filter and
+// scatter, warp 8 only moves data.  One lane of it copies each whole tile of every column slot with the
+// bulk-copy unit (cp.async.bulk, evict-first) into a ring of D stages, gated by a full / empty mbarrier
+// pair per stage.  The consumers read a stage into registers and hand it back at once.  So the ring is
+// refilled while they filter, stash, and copy the survivors out, and D tiles of reads stay in flight
+// through a copy-out; the plain kernel has one prefetched tile then.  The ring also frees the registers
+// and the second CTA the plain kernel needs to hide its loads, which leaves room for a larger stash and
+// so longer store runs per partition.  A bulk copy needs a 16-byte aligned source: the host runs this
+// kernel only when every column slot starts 16-byte aligned.  A partial last tile is loaded with
+// load_slot, so no copy reads past a column.
+constexpr int kRingThreads = kBlock + 32;
+constexpr size_t kRingSlotBytes = (size_t)kTileRows * 8;  // one slot of a stage: one tile of the widest column
+constexpr size_t kRingSmemBudget = 209 << 10;             // dynamic shared memory: 227 KB less the 17.1 KB of static arrays
+template <int NS>
+__host__ __device__ constexpr int ring_stages() { return NS <= 4 ? 3 : 2; }
+template <int NS>
+__host__ __device__ constexpr size_t ring_bytes() { return (size_t)ring_stages<NS>() * NS * kRingSlotBytes; }
+// the stash takes the rest, in multiples of 256 rows, at most 8192 (NS = 1 .. 8: 8192, 7424, 4608, 2816, 2816, 2048, 1536, 1024)
+template <int NS>
+__host__ __device__ constexpr int ring_stash_rows() {
+  return (kRingSmemBudget - 128 - ring_bytes<NS>()) / (8 * NS + 6) / 256 * 256 > 8192 ? 8192
+                                                                                      : (int)((kRingSmemBudget - 128 - ring_bytes<NS>()) / (8 * NS + 6) / 256 * 256);
+}
+template <int NS>
+__host__ __device__ constexpr size_t ring_smem_bytes() { return 128 + ring_bytes<NS>() + (size_t)ring_stash_rows<NS>() * (8 * NS + 4 + 2); }
+
+// The thread's kRowsPerThread rows of one column tile in a ring stage, widened as load_slot widens them.
+__device__ __forceinline__ void ring_slot(const unsigned char* st, int dt, RowVals& out) {
+  const int t = threadIdx.x;
+  if (dt == DBX_I64 || dt == DBX_U64 || dt == DBX_F64) {
+    const ulonglong2 a = reinterpret_cast<const ulonglong2*>(st)[2 * t], b = reinterpret_cast<const ulonglong2*>(st)[2 * t + 1];
+    out.v[0] = a.x; out.v[1] = a.y; out.v[2] = b.x; out.v[3] = b.y;
+  } else if (dt == DBX_I32 || dt == DBX_U32 || dt == DBX_F32) {
+    const uint4 q = reinterpret_cast<const uint4*>(st)[t];
+    const uint32_t w[kRowsPerThread] = {q.x, q.y, q.z, q.w};
 #pragma unroll
-      for (int s = 0; s < NS; ++s) po.out[s][d] = stash[(size_t)s * R + i];
+    for (int j = 0; j < kRowsPerThread; ++j)
+      out.v[j] = dt == DBX_I32 ? widen<int32_t>((int32_t)w[j]) : (dt == DBX_U32 ? (uint64_t)w[j] : f32_bits_to_f64_bits(w[j]));
+  } else if (dt == DBX_I16 || dt == DBX_U16) {
+    const uint64_t q = reinterpret_cast<const uint64_t*>(st)[t];
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j) {
+      const uint16_t w = (uint16_t)(q >> (16 * j));
+      out.v[j] = dt == DBX_I16 ? widen<int16_t>((int16_t)w) : (uint64_t)w;
     }
-    for (int r = threadIdx.x; r < po.n_parts; r += kBlock) s_cnt[r] = 0;
-    n_stash = 0;
-    __syncthreads();  // shared buffers are reused by the next tiles
+  } else {  // DBX_I8, DBX_U8: the host sends no other type through the ring
+    const uint32_t q = reinterpret_cast<const uint32_t*>(st)[t];
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j) {
+      const uint8_t w = (uint8_t)(q >> (8 * j));
+      out.v[j] = dt == DBX_I8 ? widen<int8_t>((int8_t)w) : (uint64_t)w;
+    }
+  }
+}
+
+template <int NS, bool EXPR = false>
+__device__ __forceinline__ void filter_partition_ring_body(const AggKernelParams& p, const PartitionOut& po) {
+  constexpr int R = ring_stash_rows<NS>();
+  constexpr int D = ring_stages<NS>();
+  static_assert(R >= kTileRows, "the stash holds at least one tile");
+  // dynamic shared memory: [D] full and [D] empty barriers (128 B), the ring [D][NS][kRingSlotBytes], then the
+  // stash as in filter_partition_body
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw);  // completes when the stage holds its tile
+  uint64_t* empty = full + D;                               // completes when every consumer warp has read the stage
+  unsigned char* ring = smem_raw + 128;
+  uint64_t* stash = reinterpret_cast<uint64_t*>(ring + ring_bytes<NS>());
+  uint32_t* tag = reinterpret_cast<uint32_t*>(stash + (size_t)NS * R);
+  uint16_t* perm = reinterpret_cast<uint16_t*>(tag + R);
+  __shared__ unsigned int s_cnt[kMaxPartitions];
+  __shared__ unsigned int s_off[kMaxPartitions];
+  __shared__ unsigned long long s_base[kMaxPartitions];
+  __shared__ unsigned int s_wcnt[2][kWarpsPerBlock];
+  const int64_t n_tiles = (p.n_rows + kTileRows - 1) / kTileRows;
+  const int64_t n_full = p.n_rows / kTileRows;  // whole tiles come through the ring
+  if (threadIdx.x == 0) {
+    for (int d = 0; d < D; ++d) { mbar_init(&full[d], 1); mbar_init(&empty[d], kWarpsPerBlock); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int r = threadIdx.x; r < po.n_parts; r += kRingThreads) s_cnt[r] = 0;
+  __syncthreads();  // the last CTA-wide barrier: from here on the consumers synchronise on barrier 1 only
+  if (threadIdx.x >= kBlock) {  // the producer warp
+    if (threadIdx.x == kBlock) {
+      const uint64_t pol = make_policy_evict_first();
+      uint32_t tile_bytes = 0;
+#pragma unroll
+      for (int s = 0; s < NS; ++s)
+        if (!p.cols[s].is_const) tile_bytes += kTileRows * dtype_size(p.cols[s].dtype);
+      int k = 0;
+      for (int64_t tile = blockIdx.x; tile < n_full; tile += gridDim.x, ++k) {
+        const int st = k % D;
+        mbar_wait(&empty[st], ((k / D) & 1) ^ 1);  // the first round finds every stage free
+        mbar_expect_tx(&full[st], tile_bytes);
+#pragma unroll
+        for (int s = 0; s < NS; ++s) {
+          if (p.cols[s].is_const) continue;
+          const int w = dtype_size(p.cols[s].dtype);
+          bulk_copy_g2s(ring + ((size_t)st * NS + s) * kRingSlotBytes, (const char*)p.cols[s].data + tile * kTileRows * w,
+                        (uint32_t)(kTileRows * w), &full[st], pol);
+        }
+      }
+    }
+    return;
+  }
+  const uint64_t pol = make_policy_evict_first();
+  int n_stash = 0;  // uniform over the consumer threads
+  int parity = 0;
+  RowVals vals[NS];
+  uint32_t vmask[NS];
+  int k = 0;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++k) {
+    if (tile < n_full) {
+      const int st = k % D;
+      mbar_wait(&full[st], (k / D) & 1);
+#pragma unroll
+      for (int s = 0; s < NS; ++s) {
+        if (p.cols[s].is_const) load_slot<false>(p.cols[s], tile * kTileRows, p.n_rows, nullptr, pol, vals[s], vmask[s]);
+        else { ring_slot(ring + ((size_t)st * NS + s) * kRingSlotBytes, p.cols[s].dtype, vals[s]); vmask[s] = 0xF; }
+      }
+      __syncwarp();
+      if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[st]);  // the stage is in registers: the producer may refill it
+    } else {
+#pragma unroll
+      for (int s = 0; s < NS; ++s) load_slot<false>(p.cols[s], tile * kTileRows, p.n_rows, nullptr, pol, vals[s], vmask[s]);
+    }
+    partition_stash_tile<NS, EXPR, R, 1>(p, po, vals, vmask, tile * kTileRows, stash, tag, s_cnt, s_wcnt, n_stash, parity);
+    if (n_stash + kTileRows <= R && tile + gridDim.x < n_tiles) continue;
+    partition_copy_out<NS, R, 1>(po, stash, tag, perm, s_cnt, s_off, s_base, n_stash);
   }
 }
 
@@ -1288,6 +1447,11 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
 template <int NS, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock, 2) filter_partition_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ PartitionOut po) {
   filter_partition_body<NS, EXPR>(p, po);
+}
+template <int NS, bool EXPR = false>
+__global__ void __launch_bounds__(kRingThreads, 1) filter_partition_ring_kernel(const __grid_constant__ AggKernelParams p,
+                                                                                const __grid_constant__ PartitionOut po) {
+  filter_partition_ring_body<NS, EXPR>(p, po);
 }
 template <int NS>
 __global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ SliceIn si) {

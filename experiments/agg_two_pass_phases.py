@@ -1,8 +1,11 @@
 """Times the phases of the two-pass aggregation of configs[1] (filter v % 3 = 0, sum / count / avg GROUP BY k)
 separately: pass 1 (filter_partition_kernel, or its build for the plan dbx_jit_agg_part), pass 2 (slice_agg_kernel or
 dbx_jit_agg_slice, or the fused kernel per L2 region for tables with too many slices) and the deferred rows (the fused kernel over a row list), each against its byte
-floor at the data-sheet HBM bandwidth.  Kernel times come from torch.profiler (CUDA activities) over `steps`
-queries after one warm-up query; the card's name and power limit are printed with them.
+floor at the data-sheet HBM bandwidth and at the copy rate this card reaches (a device-to-device torch copy_
+that reads and writes 4 GiB each, best of five, timed with CUDA events).  Kernel times come from torch.profiler
+(CUDA activities) over `steps` queries after one warm-up query; the card's name, power limit and SM clock are
+printed with them, and the operator's variant text says which pass-1 kernel ran (DBX_AGG_PART_RING=0: the
+plain kernel instead of the bulk-copy ring).
 usage: python experiments/agg_two_pass_phases.py [rows] [n_keys] [steps]"""
 import collections
 import ctypes as C
@@ -49,6 +52,25 @@ part = TransformPartialAggregate(params, types, filt)
 fin = TransformFinalAggregate(params, types)
 
 
+def copy_rate():
+    """bytes per second a device-to-device copy moves (read + write) on this card"""
+    n = 4 << 30
+    src = torch.empty(n, dtype=torch.uint8, device="cuda:0").fill_(1)
+    dst = torch.empty_like(src)
+    dst.copy_(src)
+    best = float("inf")
+    for _ in range(5):
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0.record()
+        dst.copy_(src)
+        t1.record()
+        t1.synchronize()
+        best = min(best, t0.elapsed_time(t1) / 1e3)
+    del src, dst
+    torch.cuda.empty_cache()
+    return 2 * n / best
+
+
 def query():
     part.reset(); fin.reset()
     part.transform(blk)
@@ -59,6 +81,7 @@ def query():
     return g
 
 
+copy_bytes_per_s = copy_rate()
 query()
 torch.cuda.synchronize()
 with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
@@ -69,7 +92,7 @@ ms = collections.defaultdict(float)
 for e in prof.events():
     if e.device_type == torch.autograd.DeviceType.CUDA:
         name = e.name
-        if "filter_partition_kernel" in name or "dbx_jit_agg_part" in name:
+        if "filter_partition_kernel" in name or "filter_partition_ring_kernel" in name or "dbx_jit_agg_part" in name:
             key = "pass1 filter_partition_kernel"
         elif "slice_agg_kernel" in name or "dbx_jit_agg_slice" in name:
             key = "pass2 slice_agg_kernel"
@@ -84,12 +107,18 @@ variant = part.kernel_variant()
 part.close(); fin.close()
 table_bytes = (2 ** 21 + 2) * 32  # config 2's default table: 2^21 slots x (key + 3 state words)
 chunks = (rows + (1 << 28) - 1) >> 28
-floors = {
-    "pass1 filter_partition_kernel": (24 * rows + 24 * survivors) / HBM_BYTES_PER_S * 1e3,
-    "pass2 slice_agg_kernel": (24 * survivors + 2 * table_bytes * chunks) / HBM_BYTES_PER_S * 1e3,
+moved = {
+    "pass1 filter_partition_kernel": 24 * rows + 24 * survivors,
+    "pass2 slice_agg_kernel": 24 * survivors + 2 * table_bytes * chunks,
 }
+floors = {k: b / HBM_BYTES_PER_S * 1e3 for k, b in moved.items()}
+copy_floors = {k: b / copy_bytes_per_s * 1e3 for k, b in moved.items()}
+ring = variant.split("pass 1 on the bulk-copy ring: ")[1].split(";")[0] if "bulk-copy ring" in variant else "n/a"
 report = {"card": card, "rows": rows, "keys": n_keys, "survivors": survivors, "groups": groups, "steps": steps, "kernel_variant": variant,
+          "pass1_on_ring": ring, "copy_rate_TB/s": round(copy_bytes_per_s / 1e12, 3),
           "ms_per_query": {k: round(x, 3) for k, x in sorted(ms.items())},
           "floor_ms_at_3.35TB/s": {k: round(x, 3) for k, x in floors.items()},
-          "share_of_floor": {k: round(floors[k] / ms[k], 3) for k in floors if ms.get(k)}}
+          "share_of_floor": {k: round(floors[k] / ms[k], 3) for k in floors if ms.get(k)},
+          "floor_ms_at_copy_rate": {k: round(x, 3) for k, x in copy_floors.items()},
+          "share_of_copy_rate_floor": {k: round(copy_floors[k] / ms[k], 3) for k in copy_floors if ms.get(k)}}
 print(json.dumps(report, indent=1), flush=True)

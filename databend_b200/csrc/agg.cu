@@ -10,6 +10,7 @@
 //   AggregateHashTable                 src/query/expression/src/aggregate/aggregate_hashtable.rs:168-408
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 #include "agg_kernels.cuh"
 #include "agg_jit.h"
@@ -22,7 +23,6 @@ namespace {
 constexpr int64_t kChunkRows = 1LL << 28;        // rows per kernel launch (u32 overflow row ids)
 constexpr int64_t kDefaultTableBytes = 64 << 20; // default table: 1e6 groups of config 2's shape without growth
 constexpr int kProbeLimit = 64;  // buckets (x4 slots)
-constexpr uint32_t kDefaultBulkLanes = 0x6DB6DB6Du;  // 21 of 32 lanes on the TMA unit
 
 inline int grid_for_rows(int64_t n_rows) {
   int64_t tiles = (n_rows + kTileRows - 1) / kTileRows;
@@ -79,15 +79,7 @@ struct AggPlan {
   int n_updates = 0;
   UpdateDev upd[kMaxUpdates];
   FinalAgg fin[DBX_MAX_AGGS];  // out pointers filled at finalize time
-  // state layout: words that are updated in pairs by one TMA bulk reduction sit in arrays of
-  // 16-byte pairs; w_pair[w] = pair index or -1, w_pos[w] = 0/1 position inside the pair
-  int n_pairs = 0;
-  PairDev pairs[kMaxPairs];
-  int w_pair[kMaxWords];
-  int w_pos[kMaxWords];
   // tuning knobs, read from the environment once per operator (experiments sweep them in one process)
-  uint32_t bulk_lanes = 0;   // lanes of a warp that update pairs through the TMA unit (the rest use REDs)
-  bool use_ring = true;      // ring kernel for the straight-line case with pairs
   bool l2_persist = true;    // persisting L2 access-policy window over the table
   int debug_flags = 0;
   bool hot_cache = false;    // per-CTA shared-memory cache of hot groups (skewed keys); DBX_AGG_HOT=0 turns it off
@@ -488,7 +480,7 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
   memset(&pl->init, 0, sizeof(pl->init));
   memset(&pl->kinds, 0, sizeof(pl->kinds));
   pl->add_word(0, UPD_ADD_INT);
-  pl->upd[pl->n_updates++] = UpdateDev{UPD_INC, 0, 0, 0, 0, 0};
+  pl->upd[pl->n_updates++] = UpdateDev{UPD_INC, 0, 0, 0};
   int cnt_word_of_col[kMaxCols], acc_word_of_col[kMaxCols];
   for (int i = 0; i < kMaxCols; ++i) cnt_word_of_col[i] = acc_word_of_col[i] = -1;
 
@@ -516,7 +508,7 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
     } else {
       if (cnt_word_of_col[ad.arg_col] < 0) {
         cnt_word_of_col[ad.arg_col] = pl->add_word(0, UPD_ADD_INT);
-        pl->upd[pl->n_updates++] = UpdateDev{UPD_INC_VALID, slot, cnt_word_of_col[ad.arg_col], 0, 0, 0};
+        pl->upd[pl->n_updates++] = UpdateDev{UPD_INC_VALID, slot, cnt_word_of_col[ad.arg_col], 0};
       }
       fa.cnt_word = cnt_word_of_col[ad.arg_col];
     }
@@ -528,7 +520,7 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
         if (acc_word_of_col[ad.arg_col] < 0) {
           int op = cls == VC_FLT ? UPD_ADD_F64 : UPD_ADD_INT;
           acc_word_of_col[ad.arg_col] = pl->add_word(0, op);
-          pl->upd[pl->n_updates++] = UpdateDev{op, slot, acc_word_of_col[ad.arg_col], 0, 0, 0};
+          pl->upd[pl->n_updates++] = UpdateDev{op, slot, acc_word_of_col[ad.arg_col], 0};
         }
         fa.acc_word = acc_word_of_col[ad.arg_col];
         break;
@@ -538,7 +530,7 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
         int op = cls == VC_FLT ? (mn ? UPD_MIN_F64 : UPD_MAX_F64) : cls == VC_UINT ? (mn ? UPD_MIN_U64 : UPD_MAX_U64) : (mn ? UPD_MIN_S64 : UPD_MAX_S64);
         uint64_t iv = op == UPD_MIN_S64 ? (uint64_t)INT64_MAX : op == UPD_MAX_S64 ? (uint64_t)INT64_MIN : (op == UPD_MIN_U64 || op == UPD_MIN_F64) ? ~0ULL : 0ULL;
         fa.acc_word = pl->add_word(iv, op);
-        pl->upd[pl->n_updates++] = UpdateDev{op, slot, fa.acc_word, 0, 0, 0};
+        pl->upd[pl->n_updates++] = UpdateDev{op, slot, fa.acc_word, 0};
         break;
       }
       default: err->set("unknown aggregate kind"); return DBX_ERR_INVALID;
@@ -549,41 +541,8 @@ int32_t build_plan(const dbx_agg_params* p, const int32_t* types, int32_t n_cols
     pl->slot_of(0, err);
   }
   if (pl->n_comp) DBX_TRY(allocate_slots(pl, err));
-  // Pair up additive words of the same class (integer adds incl. counters, or f64 adds), in
-  // plan order: each pair costs one L2 reduction per row instead of two (the table phase is
-  // bound by L2 atomic operations per row, not by bytes).
-  for (int w = 0; w < kMaxWords; ++w) { pl->w_pair[w] = -1; pl->w_pos[w] = 0; }
-  pl->n_pairs = 0;
-  // The TMA bulk-reduction path does not lift the bound: a 16-byte bulk reduction is split into
-  // two 8-byte L2 atomic operations, and the L2 atomic units are what the kernel is bound by.
-  // The pair layout and the ring kernel therefore stay opt-in (DBX_AGG_BULK=1); the default is
-  // one RED per state word.
-  const char* bulk_env = getenv("DBX_AGG_BULK");
-  if (pl->grouped && bulk_env && atoi(bulk_env) != 0) {
-    for (int cls = 0; cls < 2 && pl->n_pairs < kMaxPairs; ++cls) {
-      int pending = -1;
-      for (int u = 0; u < pl->n_updates && pl->n_pairs < kMaxPairs; ++u) {
-        const int op = pl->upd[u].op;
-        const bool is_int = op == UPD_INC || op == UPD_INC_VALID || op == UPD_ADD_INT;
-        const bool is_f64 = op == UPD_ADD_F64;
-        if (!(cls == 0 ? is_int : is_f64)) continue;
-        if (pending < 0) { pending = u; continue; }
-        PairDev& pd = pl->pairs[pl->n_pairs];
-        pd.upd0 = pending; pd.upd1 = u; pd.is_f64 = cls; pd.pad = 0;
-        pl->w_pair[pl->upd[pending].word] = pl->n_pairs; pl->w_pos[pl->upd[pending].word] = 0;
-        pl->w_pair[pl->upd[u].word] = pl->n_pairs; pl->w_pos[pl->upd[u].word] = 1;
-        pl->upd[pending].paired = 1;
-        pl->upd[u].paired = 1;
-        pl->n_pairs += 1;
-        pending = -1;
-      }
-    }
-  }
-  // Lane split between the TMA unit and the RED path (experiments/agg_sweep.py sweeps it).
-  pl->bulk_lanes = getenv("DBX_AGG_BULK_LANES") ? (uint32_t)strtoul(getenv("DBX_AGG_BULK_LANES"), nullptr, 16) : kDefaultBulkLanes;
-  pl->use_ring = !(getenv("DBX_AGG_RING") && atoi(getenv("DBX_AGG_RING")) == 0);
   pl->debug_flags = getenv("DBX_AGG_DEBUG") ? atoi(getenv("DBX_AGG_DEBUG")) : 0;
-  pl->hot_cache = pl->grouped && pl->key_words == 1 && pl->n_pairs == 0 && pl->n_words <= kHotWords &&
+  pl->hot_cache = pl->grouped && pl->key_words == 1 && pl->n_words <= kHotWords &&
                   !(getenv("DBX_AGG_HOT") && atoi(getenv("DBX_AGG_HOT")) == 0);
   pl->l2_persist = !(getenv("DBX_AGG_L2_PERSIST") && atoi(getenv("DBX_AGG_L2_PERSIST")) == 0);
   return DBX_OK;
@@ -598,10 +557,7 @@ struct DeviceTable {
   DevBuf counters;  // [0] n_groups, [1] n_overflow
   int64_t cap = 0;
   int n_words = 0;
-  int n_pairs = 0;
   int key_words = 1;
-  int w_pair[kMaxWords];
-  int w_pos[kMaxWords];
 
   unsigned long long* n_groups() const { return (unsigned long long*)counters.p; }
   unsigned long long* n_overflow() const { return (unsigned long long*)counters.p + 1; }
@@ -610,10 +566,7 @@ struct DeviceTable {
   int32_t create(int64_t capacity, const AggPlan& pl, cudaStream_t stream, ErrorSink* err) {
     cap = capacity < 4 ? 4 : capacity;
     n_words = pl.n_words;
-    n_pairs = pl.n_pairs;
     key_words = pl.key_words;
-    memcpy(w_pair, pl.w_pair, sizeof(w_pair));
-    memcpy(w_pos, pl.w_pos, sizeof(w_pos));
     const size_t kbytes = ((size_t)(cap + 2) * 8 * key_words + 32 + 255) & ~(size_t)255;
     DBX_CUDA_TRY(*err, mem.ensure(kbytes + (size_t)(cap + 2) * 8 * n_words));
     keys_p = mem.p;
@@ -643,22 +596,6 @@ struct DeviceTable {
     t.cap = cap;
     t.n_words = n_words;
     t.key_words = key_words;
-    // pair arrays first (16-byte aligned: every region has an even number of words), then the
-    // unpaired words row-major (one entry per slot, so a row's REDs fall into 1-2 sectors)
-    {
-      const int64_t n_slots = cap + 2;
-      const int64_t row_base = 2 * n_slots * n_pairs;
-      int n_single = 0;
-      for (int w = 0; w < n_words; ++w) n_single += w_pair[w] < 0;
-      for (int w = 0; w < kMaxWords; ++w) { t.w_off[w] = 0; t.w_stride[w] = 1; }
-      t.row_base = row_base;
-      t.n_single = n_single;
-      int idx = 0;
-      for (int w = 0; w < n_words; ++w) {
-        if (w_pair[w] >= 0) { t.w_off[w] = 2 * n_slots * w_pair[w] + w_pos[w]; t.w_stride[w] = 2; }
-        else { t.w_off[w] = row_base + idx++; t.w_stride[w] = n_single; }
-      }
-    }
     t.n_groups = n_groups();
     t.n_overflow = n_overflow();
     t.overflow_rows = overflow_rows;
@@ -675,10 +612,7 @@ struct DeviceTable {
     std::swap(counters, o.counters);
     std::swap(cap, o.cap);
     std::swap(n_words, o.n_words);
-    std::swap(n_pairs, o.n_pairs);
     std::swap(key_words, o.key_words);
-    std::swap(w_pair, o.w_pair);
-    std::swap(w_pos, o.w_pos);
   }
 };
 
@@ -692,36 +626,28 @@ inline int64_t next_pow2(int64_t x) {
 
 static std::atomic<size_t> g_persist_limit[64];  // cudaLimitPersistingL2CacheSize as last set, per device
 
-// sizeof(StageWarp<NS>) for a run-time slot count
-static size_t kMaxSlotsStageBytes(int ns) {
+// calls f(std::integral_constant<int, NS>) for a run-time slot count (1..8; anything else: 8)
+template <class F>
+static auto by_slots(int ns, F&& f) {
   switch (ns) {
-    case 1: return sizeof(StageWarp<1>); case 2: return sizeof(StageWarp<2>); case 3: return sizeof(StageWarp<3>); case 4: return sizeof(StageWarp<4>);
-    case 5: return sizeof(StageWarp<5>); case 6: return sizeof(StageWarp<6>); case 7: return sizeof(StageWarp<7>); default: return sizeof(StageWarp<8>);
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 3: return f(std::integral_constant<int, 3>());
+    case 4: return f(std::integral_constant<int, 4>());
+    case 5: return f(std::integral_constant<int, 5>());
+    case 6: return f(std::integral_constant<int, 6>());
+    case 7: return f(std::integral_constant<int, 7>());
+    default: return f(std::integral_constant<int, 8>());
   }
 }
 
+// sizeof(StageWarp<NS>) for a run-time slot count
+static size_t kMaxSlotsStageBytes(int ns) { return by_slots(ns, [](auto s) { return sizeof(StageWarp<decltype(s)::value>); }); }
+
 // dynamic shared memory of the partitioned passes for a run-time slot count: pass 1's stash, pass 2's row buffers
-static size_t partition_smem_for(int ns) {
-  switch (ns) {
-    case 1: return partition_smem_bytes<1>(); case 2: return partition_smem_bytes<2>(); case 3: return partition_smem_bytes<3>();
-    case 4: return partition_smem_bytes<4>(); case 5: return partition_smem_bytes<5>(); case 6: return partition_smem_bytes<6>();
-    case 7: return partition_smem_bytes<7>(); default: return partition_smem_bytes<8>();
-  }
-}
-static size_t ring_smem_for(int ns) {
-  switch (ns) {
-    case 1: return ring_smem_bytes<1>(); case 2: return ring_smem_bytes<2>(); case 3: return ring_smem_bytes<3>();
-    case 4: return ring_smem_bytes<4>(); case 5: return ring_smem_bytes<5>(); case 6: return ring_smem_bytes<6>();
-    case 7: return ring_smem_bytes<7>(); default: return ring_smem_bytes<8>();
-  }
-}
-static size_t slice_stage_bytes_for(int ns) {
-  switch (ns) {
-    case 1: return slice_stage_bytes<1>(); case 2: return slice_stage_bytes<2>(); case 3: return slice_stage_bytes<3>();
-    case 4: return slice_stage_bytes<4>(); case 5: return slice_stage_bytes<5>(); case 6: return slice_stage_bytes<6>();
-    case 7: return slice_stage_bytes<7>(); default: return slice_stage_bytes<8>();
-  }
-}
+static size_t partition_smem_for(int ns) { return by_slots(ns, [](auto s) { return partition_smem_bytes<decltype(s)::value>(); }); }
+static size_t ring_smem_for(int ns) { return by_slots(ns, [](auto s) { return ring_smem_bytes<decltype(s)::value>(); }); }
+static size_t slice_stage_bytes_for(int ns) { return by_slots(ns, [](auto s) { return slice_stage_bytes<decltype(s)::value>(); }); }
 
 // ================================================================ partial
 class AggPartialOp : public Op {
@@ -737,7 +663,6 @@ class AggPartialOp : public Op {
   int64_t rows_in = 0;
   int64_t initial_cap = 0;
   bool table_ready = false;
-  bool ring_ok = false;
   bool table_clean = false;  // the exchange scatter left the table empty (fused clear): reset costs no kernel
   void* window_base = nullptr;  // L2 access-policy window currently set on the stream
   size_t window_bytes = 0;
@@ -785,19 +710,18 @@ class AggPartialOp : public Op {
                       std::to_string(part_ring_launches) + " of " + std::to_string(partitioned_chunks + partition_fallbacks);
     return variant_text.c_str();
   }
-  // Ask for kernels compiled for this plan (grouped plans without TMA pairs).  Failure is not an
+  // Ask for kernels compiled for this plan (grouped plans with 64-bit keys).  Failure is not an
   // error: the precompiled kernels serve the operator, jit_status says why.
   void specialise() {
     const char* e = getenv("DBX_AGG_JIT");
     if (e && atoi(e) == 0) { jit_status = "off (DBX_AGG_JIT=0)"; return; }
-    if (!plan.grouped || plan.n_pairs > 0 || plan.key_words != 1) { jit_status = "off (plan shape not specialised)"; return; }
+    if (!plan.grouped || plan.key_words != 1) { jit_status = "off (plan shape not specialised)"; return; }
     StaticPlan sp;
     memset(&sp, 0, sizeof(sp));
     sp.n_nodes = plan.n_nodes; sp.n_updates = plan.n_updates; sp.key_slot = plan.key_slot; sp.key_is_float = plan.key_is_float ? 1 : 0;
-    sp.n_key_parts = plan.n_key_parts; sp.debug_flags = plan.debug_flags; sp.n_single = plan.n_words; sp.hot_cache = plan.hot_cache ? 1 : 0;
+    sp.n_key_parts = plan.n_key_parts; sp.debug_flags = plan.debug_flags; sp.n_words = plan.n_words; sp.hot_cache = plan.hot_cache ? 1 : 0;
     memcpy(sp.nodes, plan.nodes, sizeof(PredNodeDev) * plan.n_nodes);
     memcpy(sp.upd, plan.upd, sizeof(UpdateDev) * plan.n_updates);
-    for (int u = 0; u < plan.n_updates; ++u) sp.upd[u].ridx = plan.upd[u].word;  // no pairs: entry index == word index
     memcpy(sp.key_parts, plan.key_parts, sizeof(plan.key_parts));
     if (plan.n_comp_ev) {
       sp.n_comp = plan.n_comp_ev; sp.comp_pred = plan.comp_pred; sp.fresh_slots = plan.fresh_slots; sp.raises = plan.can_raise ? 1 : 0;
@@ -943,50 +867,22 @@ class AggPartialOp : public Op {
     return DBX_OK;
   }
 
-  // ring kernel: whole tiles of plain 8-byte columns, pairs present, table provably large enough
-  template <int NS>
-  int32_t launch_ring(const AggKernelParams& kp) {
-    static std::atomic<bool> attr_set[64];
-    if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
-    const size_t smem = (size_t)kWarpsPerBlock * kRingCap * (16 * kp.n_pairs + 8 * kp.ring_nsv);
-    auto kern = filter_group_agg_ring_kernel<NS, 4>;
-    if (!attr_set[device]) {  // upper bound over every plan this instantiation can serve
-      const size_t smem_max = (size_t)kWarpsPerBlock * kRingCap * (16 * kMaxPairs + 8 * NS);
-      DBX_CUDA_TRY(err, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-      attr_set[device] = true;
-    }
-    int grid = grid_for_rows(kp.n_rows);
-    const int per_sm = getenv("DBX_AGG_GRID") ? atoi(getenv("DBX_AGG_GRID")) : 0;
-    if (per_sm > 0) grid = (int)std::max<int64_t>(1, std::min<int64_t>(kp.n_rows / kTileRows, (int64_t)kNumSMs * per_sm));
-    kern<<<grid, kBlock, smem, stream>>>(kp);
-    count_launch();
-    DBX_CUDA_TRY(err, cudaGetLastError());
-    return DBX_OK;
-  }
   int64_t comp_fast_launches = 0, comp_generic_launches = 0;
   template <int NS, bool FAST, bool INDIRECT>
   int32_t launch_one(const AggKernelParams& kp) {
-    // computed columns: the kernels that evaluate them (the ring and bulk variants do not: DESIGN §1, "Computed columns")
     if (kp.n_comp > 0) {
       ++(FAST ? comp_fast_launches : comp_generic_launches);
-      return launch_kernel<NS, FAST, INDIRECT, false, 4, true>(kp);
+      return launch_kernel<NS, FAST, INDIRECT, true>(kp);
     }
-    // the TMA bulk-reduction variants exist for the straight-line kernel only; everywhere else
-    // paired words are updated with plain REDs
-    if (FAST && !INDIRECT && kp.n_pairs > 0 && plan.use_ring && ring_ok) return launch_ring<NS>(kp);
-    if (FAST && !INDIRECT && kp.n_pairs > 0 && getenv("DBX_AGG_BULK_OLD")) return launch_kernel<NS, FAST, INDIRECT, true, 4>(kp);
-    // (4 CTAs/SM at 62 registers: 5-6 CTAs spill and queue up behind the L2 atomics, 2-3 CTAs hide
-    // less latency)
-    return launch_kernel<NS, FAST, INDIRECT, false, 4>(kp);
+    return launch_kernel<NS, FAST, INDIRECT>(kp);
   }
-  template <int NS, bool FAST, bool INDIRECT, bool BULK, int MINB, bool EXPR = false>
+  template <int NS, bool FAST, bool INDIRECT, bool EXPR = false>
   int32_t launch_kernel(const AggKernelParams& kp) {
     static std::atomic<bool> attr_set[64];
     if (device < 0 || device >= 64) { err.set("device index out of range"); return DBX_ERR_INVALID; }
-    const size_t smem_rows = (sizeof(StageWarp<NS>) * kWarpsPerBlock + 15) & ~(size_t)15;
-    const size_t smem_bulk = (size_t)kWarpsPerBlock * kBulkGen * kMaxPairs * 32 * 16;
-    const size_t smem = smem_rows + (BULK ? smem_bulk : kHotBytes);  // the hot-group cache sits where the bulk staging would
-    auto kern = filter_group_agg_kernel<NS, FAST, INDIRECT, BULK, MINB, EXPR>;
+    // the row stages, then the hot-group cache
+    const size_t smem = ((sizeof(StageWarp<NS>) * kWarpsPerBlock + 15) & ~(size_t)15) + kHotBytes;
+    auto kern = filter_group_agg_kernel<NS, FAST, INDIRECT, EXPR>;
     if (!attr_set[device]) {
       DBX_CUDA_TRY(err, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       attr_set[device] = true;
@@ -995,7 +891,7 @@ class AggPartialOp : public Op {
     static const int per_sm = getenv("DBX_AGG_GRID") ? atoi(getenv("DBX_AGG_GRID")) : 0;
     if (per_sm > 0 && !(kp.table.hot_spill && per_sm > 8))  // the spill buffer of the hot-group caches is sized for 8 CTAs per SM
       grid = (int)std::max<int64_t>(1, std::min<int64_t>((kp.n_rows + kTileRows - 1) / kTileRows, (int64_t)kNumSMs * per_sm));
-    if (!BULK && !INDIRECT && jit.ok() && !no_filter_) {  // same grid, block and shared memory: only the code differs
+    if (!INDIRECT && jit.ok() && !no_filter_) {  // same grid, block and shared memory: only the code differs
       void* args[] = {(void*)&kp};
       const cudaError_t ce = cudaLaunchKernel((const void*)(FAST ? jit.fast : jit.gen), dim3(grid), dim3(kBlock), args, smem, stream);
       if (ce == cudaSuccess) { count_launch(); return DBX_OK; }
@@ -1024,33 +920,14 @@ class AggPartialOp : public Op {
   }
   template <bool INDIRECT>
   int32_t launch_wide_ns(const AggKernelParams& kp) {
-    return kp.n_comp > 0 ? launch_wide_slots<INDIRECT, true>(kp) : launch_wide_slots<INDIRECT, false>(kp);
-  }
-  template <bool INDIRECT, bool EXPR>
-  int32_t launch_wide_slots(const AggKernelParams& kp) {
-    switch (plan.n_slots) {
-      case 1: return launch_wide<1, INDIRECT, EXPR>(kp);
-      case 2: return launch_wide<2, INDIRECT, EXPR>(kp);
-      case 3: return launch_wide<3, INDIRECT, EXPR>(kp);
-      case 4: return launch_wide<4, INDIRECT, EXPR>(kp);
-      case 5: return launch_wide<5, INDIRECT, EXPR>(kp);
-      case 6: return launch_wide<6, INDIRECT, EXPR>(kp);
-      case 7: return launch_wide<7, INDIRECT, EXPR>(kp);
-      default: return launch_wide<8, INDIRECT, EXPR>(kp);
-    }
+    return by_slots(plan.n_slots, [&](auto s) {
+      constexpr int NS = decltype(s)::value;
+      return kp.n_comp > 0 ? launch_wide<NS, INDIRECT, true>(kp) : launch_wide<NS, INDIRECT, false>(kp);
+    });
   }
   template <bool FAST, bool INDIRECT>
   int32_t launch_ns(const AggKernelParams& kp) {
-    switch (plan.n_slots) {
-      case 1: return launch_one<1, FAST, INDIRECT>(kp);
-      case 2: return launch_one<2, FAST, INDIRECT>(kp);
-      case 3: return launch_one<3, FAST, INDIRECT>(kp);
-      case 4: return launch_one<4, FAST, INDIRECT>(kp);
-      case 5: return launch_one<5, FAST, INDIRECT>(kp);
-      case 6: return launch_one<6, FAST, INDIRECT>(kp);
-      case 7: return launch_one<7, FAST, INDIRECT>(kp);
-      default: return launch_one<8, FAST, INDIRECT>(kp);
-    }
+    return by_slots(plan.n_slots, [&](auto s) { return launch_one<decltype(s)::value, FAST, INDIRECT>(kp); });
   }
   // The straight-line variant applies to plain 8-byte device columns (no validity, 32 B aligned)
   // with at most one Compare; it covers whole tiles, the generic kernel takes the remainder.
@@ -1085,23 +962,13 @@ class AggPartialOp : public Op {
     }
     return DBX_OK;
   }
-  template <bool EXPR>
-  void launch_single_slots(const AggKernelParams& kp, int grid) {
-    switch (plan.n_slots) {
-      case 1: filter_single_agg_kernel<1, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 2: filter_single_agg_kernel<2, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 3: filter_single_agg_kernel<3, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 4: filter_single_agg_kernel<4, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 5: filter_single_agg_kernel<5, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 6: filter_single_agg_kernel<6, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      case 7: filter_single_agg_kernel<7, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-      default: filter_single_agg_kernel<8, EXPR><<<grid, kBlock, 0, stream>>>(kp); break;
-    }
-  }
   int32_t launch_single(const AggKernelParams& kp) {
     int grid = std::min(grid_for_rows(kp.n_rows), kNumSMs * 4);
-    if (kp.n_comp > 0) launch_single_slots<true>(kp, grid);
-    else launch_single_slots<false>(kp, grid);
+    by_slots(plan.n_slots, [&](auto s) {
+      constexpr int NS = decltype(s)::value;
+      if (kp.n_comp > 0) filter_single_agg_kernel<NS, true><<<grid, kBlock, 0, stream>>>(kp);
+      else filter_single_agg_kernel<NS, false><<<grid, kBlock, 0, stream>>>(kp);
+    });
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
     return DBX_OK;
@@ -1120,11 +987,6 @@ class AggPartialOp : public Op {
     }
     memcpy(kp->nodes, plan.nodes, sizeof(PredNodeDev) * plan.n_nodes);
     memcpy(kp->upd, plan.upd, sizeof(UpdateDev) * plan.n_updates);
-    for (int u = 0; u < plan.n_updates; ++u) {  // position of an unpaired word inside the row-major entry
-      int idx = 0;
-      for (int w = 0; w < plan.upd[u].word; ++w) idx += plan.w_pair[w] < 0;
-      kp->upd[u].ridx = idx;
-    }
     kp->n_rows = n;
     kp->n_slots = plan.n_slots;
     kp->n_nodes = no_filter_ ? 0 : plan.n_nodes;  // pass 2 of the partitioned path: the rows are the survivors already
@@ -1134,20 +996,7 @@ class AggPartialOp : public Op {
     kp->key_is_float = plan.key_is_float ? 1 : 0;
     kp->n_key_parts = plan.n_key_parts;
     memcpy(kp->key_parts, plan.key_parts, sizeof(plan.key_parts));
-    kp->n_pairs = plan.n_pairs;
-    memcpy(kp->pairs, plan.pairs, sizeof(PairDev) * kMaxPairs);
-    kp->bulk_lanes = plan.bulk_lanes;
     kp->debug_flags = plan.debug_flags;
-    // ring kernel: slots the table phase reads back from the ring = key parts + arguments of unpaired updates
-    bool need[kMaxSlots] = {};
-    if (plan.n_key_parts > 1) for (int j = 0; j < plan.n_key_parts; ++j) need[plan.key_parts[j].slot] = true;
-    else if (plan.key_slot >= 0) need[plan.key_slot] = true;
-    for (int u = 0; u < plan.n_updates; ++u) {
-      const UpdateDev& ud = plan.upd[u];
-      if (!ud.paired && ud.op != UPD_INC && ud.op != UPD_INC_VALID) need[ud.slot] = true;
-    }
-    kp->ring_nsv = 0;
-    for (int s = 0; s < kMaxSlots; ++s) kp->ring_sidx[s] = (s < plan.n_slots && need[s]) ? (int8_t)kp->ring_nsv++ : (int8_t)-1;
     // computed columns, except over pass 1's buffers (they hold the computed values already)
     if (plan.n_comp_ev && !no_filter_) {
       kp->n_comp = plan.n_comp_ev;
@@ -1260,7 +1109,7 @@ class AggPartialOp : public Op {
   static constexpr int64_t kPartChunkRows = 1LL << 28;
   static constexpr int kMaxRegions = 64;  // partitions of the L2-region pass 2
   bool partition_eligible(const DevCol* cols, int64_t m) const {
-    if (!plan.grouped || plan.key_words != 1 || plan.n_pairs > 0 || part_threshold <= 0) return false;
+    if (!plan.grouped || plan.key_words != 1 || part_threshold <= 0) return false;
     if ((int64_t)table.bytes() <= part_threshold || m < (1 << 16)) return false;
     // every partition pass pulls its table region into L2 again: worth it only when the rows outweigh the table
     if (m * 8 * plan.n_slots < 4 * (int64_t)table.bytes() && !getenv("DBX_AGG_PARTITION_ALWAYS")) return false;
@@ -1432,12 +1281,7 @@ class AggPartialOp : public Op {
     DBX_CUDA_TRY(err, cudaMemsetAsync(part_cnt.p, 0, (kMaxPartitions + 1) * 8, stream));
     po.counts = (unsigned long long*)part_cnt.p; po.cap_p = cap_p; po.nb_mask = (uint64_t)(nb - 1);
     po.region_shift = lg_nb - lg_p; po.n_parts = n_parts;
-    switch (plan.n_slots) {
-      case 1: DBX_TRY(launch_partition<1>(kp, po)); break; case 2: DBX_TRY(launch_partition<2>(kp, po)); break;
-      case 3: DBX_TRY(launch_partition<3>(kp, po)); break; case 4: DBX_TRY(launch_partition<4>(kp, po)); break;
-      case 5: DBX_TRY(launch_partition<5>(kp, po)); break; case 6: DBX_TRY(launch_partition<6>(kp, po)); break;
-      case 7: DBX_TRY(launch_partition<7>(kp, po)); break; default: DBX_TRY(launch_partition<8>(kp, po)); break;
-    }
+    DBX_TRY(by_slots(plan.n_slots, [&](auto s) { return launch_partition<decltype(s)::value>(kp, po); }));
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
     DBX_CUDA_TRY(err, cudaMemcpyAsync(part_host.p, part_cnt.p, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, stream));
@@ -1467,12 +1311,7 @@ class AggPartialOp : public Op {
     si.n_deferred = (unsigned long long*)n_deferred.p;
     kp.table = table.view(nullptr);
     const size_t smem = (size_t)slice * 8 * (1 + plan.n_words);
-    switch (plan.n_slots) {
-      case 1: DBX_TRY(launch_slice_agg<1>(kp, si, n_parts, smem)); break; case 2: DBX_TRY(launch_slice_agg<2>(kp, si, n_parts, smem)); break;
-      case 3: DBX_TRY(launch_slice_agg<3>(kp, si, n_parts, smem)); break; case 4: DBX_TRY(launch_slice_agg<4>(kp, si, n_parts, smem)); break;
-      case 5: DBX_TRY(launch_slice_agg<5>(kp, si, n_parts, smem)); break; case 6: DBX_TRY(launch_slice_agg<6>(kp, si, n_parts, smem)); break;
-      case 7: DBX_TRY(launch_slice_agg<7>(kp, si, n_parts, smem)); break; default: DBX_TRY(launch_slice_agg<8>(kp, si, n_parts, smem)); break;
-    }
+    DBX_TRY(by_slots(plan.n_slots, [&](auto s) { return launch_slice_agg<decltype(s)::value>(kp, si, n_parts, smem); }));
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
     DBX_CUDA_TRY(err, cudaMemcpyAsync((char*)part_host.p + (kMaxPartitions + 1) * 8, n_deferred.p, 16, cudaMemcpyDeviceToHost, stream));
@@ -1553,7 +1392,6 @@ class AggPartialOp : public Op {
       // Insertions are provably within the load-factor budget when even "every row is a new
       // group" keeps the table at most half full: no overflow list, no host sync.
       const bool safe = (groups_known + rows_since_read + m) * 2 <= table.cap;
-      ring_ok = safe;  // the ring kernel does not record overflow rows
       if (safe) {
         kp.table = table.view(nullptr);
         if (want_hot()) { kp.hot_cache = 1; hot_probe_rows += m; }
@@ -2011,12 +1849,6 @@ class FilterOp : public Op {
   }
   int32_t reset() override { out_q.clear(); out_head = 0; rows_in = rows_out = 0; return DBX_OK; }
 
-  template <int NS>
-  void launch_select(const AggKernelParams& kp, int grid) {
-    if (kp.n_comp > 0) filter_select_kernel<NS, true><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
-    else filter_select_kernel<NS><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
-  }
-
   int32_t push(const dbx_block* b) override {
     if (b->num_cols != plan.n_cols) { err.set("push: block column count differs from the operator's input schema"); return DBX_ERR_INVALID; }
     for (int i = 0; i < plan.n_cols; ++i) {
@@ -2065,16 +1897,11 @@ class FilterOp : public Op {
       }
       const int grid = grid_for_rows(n);
       DBX_TRY(timing_begin());
-      switch (plan.n_slots) {
-        case 1: launch_select<1>(kp, grid); break;
-        case 2: launch_select<2>(kp, grid); break;
-        case 3: launch_select<3>(kp, grid); break;
-        case 4: launch_select<4>(kp, grid); break;
-        case 5: launch_select<5>(kp, grid); break;
-        case 6: launch_select<6>(kp, grid); break;
-        case 7: launch_select<7>(kp, grid); break;
-        default: launch_select<8>(kp, grid); break;
-      }
+      by_slots(plan.n_slots, [&](auto s) {
+        constexpr int NS = decltype(s)::value;
+        if (kp.n_comp > 0) filter_select_kernel<NS, true><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
+        else filter_select_kernel<NS><<<grid, kBlock, 0, stream>>>(kp, (uint8_t*)nibbles.p, (uint32_t*)tile_counts.p);
+      });
       count_launch();
       DBX_CUDA_TRY(err, cudaGetLastError());
       tile_scan_kernel<<<1, 1024, 0, stream>>>((const uint32_t*)tile_counts.p, (uint32_t*)tile_offsets.p, n_tiles);

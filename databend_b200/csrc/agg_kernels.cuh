@@ -497,15 +497,6 @@ struct StageWarp {
   uint8_t vm[kStageCap];
 };
 
-constexpr int kBulkGen = 2;  // generations of bulk-reduction staging slots per lane
-
-// value a row adds to an additive state word (0 when its argument is NULL)
-__device__ __forceinline__ uint64_t update_contribution(const UpdateDev& ud, uint64_t val, bool valid) {
-  if (ud.op == UPD_INC) return 1;
-  if (ud.op == UPD_INC_VALID) return valid ? 1 : 0;
-  return valid ? val : 0;  // UPD_ADD_INT: two's complement image; UPD_ADD_F64: +0.0 has all-zero bits
-}
-
 // ---- hot-group cache (skewed keys).  A few keys taking a large share of the rows serialise on the L2
 // atomic unit of their state words (log-uniform keys over 1e6: 57 ms instead of 7.6 ms).  Each CTA
 // therefore keeps kHotSlots groups in shared memory: a key may claim the slot its hash selects only
@@ -554,15 +545,12 @@ __device__ __forceinline__ void hot_flush_word(int op, void* w, uint64_t v) {
   red_add_u64(w, v);
 }
 
-template <int NS, bool FAST, bool BULK, int KW = 1>
+template <int NS, bool FAST, int KW = 1>
 __device__ __forceinline__ void table_phase32(const AggKernelParams& p, const StageWarp<NS>& sw, int first, int count,
-                                              int lane, uint32_t& new_groups, uint64_t* bulk_stage, int& bulk_gen,
-                                              uint64_t* hot = nullptr) {
+                                              int lane, uint32_t& new_groups, uint64_t* hot = nullptr) {
   const TableDev& t = p.table;
   const int i = first + lane;
   const bool act = lane < count;
-  const bool use_bulk = BULK && ((p.bulk_lanes >> lane) & 1);
-  int64_t good_slot = -1;
   uint64_t key = 0, key_hi = 0;
   uint32_t vm = 0xFF;
   bool key_null = false;
@@ -593,7 +581,7 @@ __device__ __forceinline__ void table_phase32(const AggKernelParams& p, const St
   const uint64_t hash = KW == 2 ? 0 : agg_hash_u64(key);
   const int64_t b = KW == 2 ? 0 : (int64_t)(hash & (uint64_t)((t.cap >> 2) - 1));
   bool cached = false;
-  if (KW == 1 && !BULK && hot) {
+  if (KW == 1 && hot) {
     const bool cand = act && !special;
     // idle lanes vote with throw-away values (a chance match only lets a key claim a slot a little earlier)
     const unsigned peers = __match_any_sync(0xffffffffu, cand ? key : (0x8000000000000001ULL + (uint64_t)lane));
@@ -632,43 +620,13 @@ __device__ __forceinline__ void table_phase32(const AggKernelParams& p, const St
       unsigned long long idx = atomicAdd(t.n_overflow, 1ULL);
       if (t.overflow_rows) t.overflow_rows[idx] = sw.row[i];
     } else if (!(PLN(debug_flags) & 1)) {
-      good_slot = slot;
-      uint64_t* row = t.states + t.row_base + slot * PLN_TABLE(n_single);
+      uint64_t* row = t.states + slot * PLN_TABLE(n_words);
       PLN_UNROLL
       for (int u = 0; u < PLN(n_updates); ++u) {
         const UpdateDev ud = PLN(upd[u]);
-        if (ud.paired) {
-          if (!use_bulk) apply_update(ud.op, word_ptr(t, slot, ud.word), sw.val[ud.slot][i], (vm >> ud.slot) & 1);
-          continue;
-        }
-        apply_update(ud.op, row + ud.ridx, sw.val[ud.slot][i], (vm >> ud.slot) & 1);
+        apply_update(ud.op, row + ud.word, sw.val[ud.slot][i], (vm >> ud.slot) & 1);
       }
     }
-  }
-  if (BULK) {
-    // Paired words: stage the row's two contributions (16 B) in shared memory and hand them to
-    // the TMA unit as one bulk reduction into the table.  The staging slots are reused every
-    // kBulkGen calls, after the bulk group that read them has drained (wait_group.read).
-    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kBulkGen - 1) : "memory");
-    if (good_slot >= 0 && use_bulk) {
-      for (int pr = 0; pr < p.n_pairs; ++pr) {
-        const PairDev pd = p.pairs[pr];
-        uint64_t* s = bulk_stage + ((size_t)(bulk_gen * kMaxPairs + pr) * 32 + lane) * 2;
-        s[0] = update_contribution(p.upd[pd.upd0], sw.val[p.upd[pd.upd0].slot][i], (vm >> p.upd[pd.upd0].slot) & 1);
-        s[1] = update_contribution(p.upd[pd.upd1], sw.val[p.upd[pd.upd1].slot][i], (vm >> p.upd[pd.upd1].slot) & 1);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      for (int pr = 0; pr < p.n_pairs; ++pr) {
-        const PairDev pd = p.pairs[pr];
-        const uint64_t* s = bulk_stage + ((size_t)(bulk_gen * kMaxPairs + pr) * 32 + lane) * 2;
-        uint64_t* dst = word_ptr(t, good_slot, p.upd[pd.upd0].word);
-        const uint32_t sa = (uint32_t)__cvta_generic_to_shared(s);
-        if (pd.is_f64) asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], 16;" ::"l"(dst), "r"(sa) : "memory");
-        else asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], 16;" ::"l"(dst), "r"(sa) : "memory");
-      }
-    }
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    bulk_gen = (bulk_gen + 1) % kBulkGen;
   }
   __syncwarp();
 }
@@ -683,18 +641,14 @@ __device__ __forceinline__ void prefetch_tile(const AggKernelParams& p, int64_t 
   }
 }
 
-template <int NS, bool FAST, bool INDIRECT, bool BULK, int KW = 1, bool EXPR = false>
+template <int NS, bool FAST, bool INDIRECT, int KW = 1, bool EXPR = false>
 __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   StageWarp<NS>& sw = reinterpret_cast<StageWarp<NS>*>(smem_raw)[warp];
-  // bulk-reduction staging: [warp][generation][pair][lane] x 16 bytes, behind the row stages
-  uint64_t* bulk_stage = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(StageWarp<NS>) * kWarpsPerBlock + 15) & ~(size_t)15)) +
-                         (size_t)warp * kBulkGen * kMaxPairs * 32 * 2;
-  int bulk_gen = 0;
   // hot-group cache behind the row stages: [kHotSlots keys][kHotSlots x kHotWords state words]
   uint64_t* hot = nullptr;
-  if (KW == 1 && !BULK && PLN(hot_cache) && p.hot_cache) {  // plan capability (compile-time when specialised) and this launch's choice
+  if (KW == 1 && PLN(hot_cache) && p.hot_cache) {  // plan capability (compile-time when specialised) and this launch's choice
     hot = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(StageWarp<NS>) * kWarpsPerBlock + 15) & ~(size_t)15));
     for (int e = threadIdx.x; e < kHotSlots; e += kBlock) {
       hot[e] = kEmptyKey;
@@ -769,12 +723,11 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
     __syncwarp();
     while (n_staged >= 32) {
       n_staged -= 32;
-      table_phase32<NS, FAST, BULK, KW>(p, sw, n_staged, 32, lane, new_groups, bulk_stage, bulk_gen, hot);
+      table_phase32<NS, FAST, KW>(p, sw, n_staged, 32, lane, new_groups, hot);
     }
   }
   __syncwarp();
-  if (n_staged > 0) table_phase32<NS, FAST, BULK, KW>(p, sw, 0, n_staged, lane, new_groups, bulk_stage, bulk_gen, hot);
-  if (BULK) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (n_staged > 0) table_phase32<NS, FAST, KW>(p, sw, 0, n_staged, lane, new_groups, hot);
   if (hot) {  // merge this CTA's cached groups into the table: one find-or-insert and one RED per word and group
     __syncthreads();
     for (int e = threadIdx.x; e < kHotSlots; e += kBlock) {
@@ -808,14 +761,15 @@ __device__ __forceinline__ void filter_group_agg_body(const AggKernelParams& p) 
 }
 
 #ifndef DBX_JIT
-template <int NS, bool FAST, bool INDIRECT, bool BULK = false, int MINB = 4, bool EXPR = false>
-__global__ void __launch_bounds__(kBlock, MINB) filter_group_agg_kernel(const __grid_constant__ AggKernelParams p) {
-  filter_group_agg_body<NS, FAST, INDIRECT, BULK, 1, EXPR>(p);
+// (4 CTAs/SM at 62 registers: 5-6 CTAs spill and queue up behind the L2 atomics, 2-3 CTAs hide less latency)
+template <int NS, bool FAST, bool INDIRECT, bool EXPR = false>
+__global__ void __launch_bounds__(kBlock, 4) filter_group_agg_kernel(const __grid_constant__ AggKernelParams p) {
+  filter_group_agg_body<NS, FAST, INDIRECT, 1, EXPR>(p);
 }
 // 128-bit packed group keys (two key words per slot): any column layout, direct or replayed rows
 template <int NS, bool INDIRECT, bool EXPR = false>
 __global__ void __launch_bounds__(kBlock, 4) filter_group_agg_wide_kernel(const __grid_constant__ AggKernelParams p) {
-  filter_group_agg_body<NS, false, INDIRECT, false, 2, EXPR>(p);
+  filter_group_agg_body<NS, false, INDIRECT, 2, EXPR>(p);
 }
 #endif
 
@@ -1323,9 +1277,8 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ unsigned int s_fill, s_fill0;  // occupied slots of the slice: now, and when it was loaded
   const TableDev& t = p.table;
-  // the two-pass path has no paired words: the nw state words of a slot are one row-major entry, and the
-  // slice's entries are one contiguous run of the table
-  const int nw = PLN_TABLE(n_single);
+  // the nw state words of a slot are one row-major entry, so the slice's entries are one contiguous run of the table
+  const int nw = PLN_TABLE(n_words);
   const int64_t S = si.slice_slots;
   uint64_t* skeys = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t* sst = skeys + S;                 // state word w of slot i at sst[i * nw + w]
@@ -1338,7 +1291,7 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
   if (threadIdx.x == 0) s_fill = s_fill0 = 0;
   __syncthreads();
   ulonglong2* gkeys = reinterpret_cast<ulonglong2*>(t.keys + slot0);
-  ulonglong2* gst = reinterpret_cast<ulonglong2*>(t.states + t.row_base + slot0 * nw);
+  ulonglong2* gst = reinterpret_cast<ulonglong2*>(t.states + slot0 * nw);
   unsigned int occupied = 0;
 #pragma unroll 2
   for (int64_t i = threadIdx.x; i < S / 2; i += kSliceBlock) {
@@ -1456,158 +1409,6 @@ __global__ void __launch_bounds__(kRingThreads, 1) filter_partition_ring_kernel(
 template <int NS>
 __global__ void __launch_bounds__(kSliceBlock, 1) slice_agg_kernel(const __grid_constant__ AggKernelParams p, const __grid_constant__ SliceIn si) {
   slice_agg_body<NS>(p, si);
-}
-
-// ---------------------------------------------------------------- fused kernel, ring variant
-// Same front end as the FAST kernel above; the table phase differs in how the state words are
-// updated.  The plain kernel is bound by the NUMBER of L2 reduction requests (experiments/
-// atomics_bench.cu), three per surviving row for config 2.  Here
-// adjacent additive words (e.g. {row count, wrapping integer sum}) are one 16-byte pair and a
-// share of the lanes updates the pair with ONE TMA bulk reduction (cp.reduce.async.bulk, a
-// separate unit that sustains ~1 small op / 5 clk / SM) while the other lanes keep using REDs,
-// so both units run side by side.  The surviving rows are compacted into a warp-private
-// shared-memory RING (FIFO) whose pair records {contribution0, contribution1} are the TMA source
-// directly — no second staging copy; a ring position is rewritten only after the bulk group that
-// read it has drained (cp.async.bulk.wait_group.read).
-//
-// Ring capacity: a tile adds <= 128 rows per warp behind < 32 carried ones, and the most recent
-// K = 1 table phases (32 rows each) may still be read by the TMA unit: R >= 128 + 31 + 32 K.
-constexpr int kRingCap = 192;
-
-template <int NS>
-__device__ __forceinline__ void ring_table_phase(const AggKernelParams& p, const uint64_t* pair_base, const uint64_t* val_base,
-                                                 int head, int count, int lane, uint32_t& new_groups) {
-  const TableDev& t = p.table;
-  const bool act = lane < count;
-  int pos = head + lane;
-  if (pos >= kRingCap) pos -= kRingCap;
-  uint64_t key = 0;
-  if (act) {
-    if (p.n_key_parts > 1) {
-      for (int j = 0; j < p.n_key_parts; ++j) {
-        const KeyPartDev kp = p.key_parts[j];
-        key |= (val_base[p.ring_sidx[kp.slot] * kRingCap + pos] & kp.mask) << kp.shift;
-      }
-    } else {
-      key = val_base[p.ring_sidx[p.key_slot] * kRingCap + pos];
-      if (p.key_is_float) key = canonical_float_key(key);
-    }
-  }
-  const bool special = key == kEmptyKey;
-  const int64_t b = (int64_t)(agg_hash_u64(key) & (uint64_t)((t.cap >> 2) - 1));
-  u64x4 kb;
-  kb.x = kb.y = kb.z = kb.w = 0;
-  if (act && !special) kb = ld_bucket(t.keys + 4 * b);
-  if (act) {
-    int64_t slot;
-    if (special) {
-      slot = special_slot(t, false, new_groups);
-    } else {
-      int m = bucket_match(kb, key);
-      slot = m >= 0 ? 4 * b + m : find_or_insert_slow(t, key, b, kb, new_groups);
-    }
-    if (slot < 0) {
-      atomicAdd(t.n_overflow, 1ULL);  // ring kernel runs in "safe" mode only: counted, reported loudly by the host
-    } else if (!(p.debug_flags & 1)) {
-      const bool use_bulk = (p.bulk_lanes >> lane) & 1;
-      uint64_t* row = t.states + t.row_base + slot * t.n_single;
-      for (int u = 0; u < p.n_updates; ++u) {
-        const UpdateDev ud = p.upd[u];
-        if (ud.paired) continue;
-        apply_update(ud.op, row + ud.ridx, (ud.op == UPD_INC || ud.op == UPD_INC_VALID) ? 0 : val_base[p.ring_sidx[ud.slot] * kRingCap + pos], true);
-      }
-      for (int pr = 0; pr < p.n_pairs; ++pr) {
-        const PairDev pd = p.pairs[pr];
-        const uint64_t* src = pair_base + ((size_t)pr * kRingCap + pos) * 2;
-        uint64_t* dst = word_ptr(t, slot, p.upd[pd.upd0].word);
-        if (use_bulk) {
-          const uint32_t sa = (uint32_t)__cvta_generic_to_shared(src);
-          if (pd.is_f64) asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], 16;" ::"l"(dst), "r"(sa) : "memory");
-          else asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], 16;" ::"l"(dst), "r"(sa) : "memory");
-        } else {
-          const uint64_t c0 = src[0], c1 = src[1];
-          if (pd.is_f64) {
-            if (c0) red_add_f64(dst, __longlong_as_double((long long)c0));
-            if (c1) red_add_f64(dst + 1, __longlong_as_double((long long)c1));
-          } else {
-            if (c0) red_add_u64(dst, c0);
-            if (c1) red_add_u64(dst + 1, c1);
-          }
-        }
-      }
-    }
-  }
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");  // every lane, every call: group counts stay aligned
-  __syncwarp();
-}
-
-template <int NS, int MINB = 4>
-__global__ void __launch_bounds__(kBlock, MINB) filter_group_agg_ring_kernel(const __grid_constant__ AggKernelParams p) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int np = p.n_pairs, nsv = p.ring_nsv;
-  const size_t warp_bytes = (size_t)kRingCap * (16 * np + 8 * nsv);
-  uint64_t* pair_base = reinterpret_cast<uint64_t*>(smem_raw + warp * warp_bytes);  // [np][kRingCap][2]
-  uint64_t* val_base = pair_base + (size_t)np * kRingCap * 2;                       // [nsv][kRingCap]
-  const int64_t n_tiles = p.n_rows / kTileRows;  // whole tiles only (the generic kernel takes the remainder)
-  const uint32_t lt_mask = (1u << lane) - 1;
-  uint32_t new_groups = 0;
-  int head = 0, cnt = 0;  // warp-uniform: the ring holds rows [head, head + cnt)
-
-  RowVals vals[NS];
-  int64_t tile = blockIdx.x;
-  if (tile < n_tiles) prefetch_tile<NS>(p, tile, vals);
-  for (; tile < n_tiles; tile += gridDim.x) {
-    __syncwarp();
-    uint32_t sel = 0xF;
-    if (p.n_nodes) {
-      const PredNodeDev& nd = p.nodes[0];
-#pragma unroll
-      for (int j = 0; j < kRowsPerThread; ++j)
-        if (!eval_cmp(nd, pick<NS>(vals, nd.l_slot, j), nd.r_const)) sel &= ~(1u << j);
-    }
-    if (p.debug_flags & 2) sel = 0;
-    // the positions written below were last handed to the TMA unit >= 2 table phases ago
-    asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < kRowsPerThread; ++j) {
-      const bool on = (sel >> j) & 1;
-      const uint32_t bal = __ballot_sync(0xffffffffu, on);
-      if (on) {
-        int o = head + cnt + __popc(bal & lt_mask);
-        if (o >= kRingCap) o -= kRingCap;
-#pragma unroll
-        for (int s = 0; s < NS; ++s)
-          if (p.ring_sidx[s] >= 0) val_base[p.ring_sidx[s] * kRingCap + o] = vals[s].v[j];
-        for (int pr = 0; pr < np; ++pr) {
-          const UpdateDev u0 = p.upd[p.pairs[pr].upd0], u1 = p.upd[p.pairs[pr].upd1];
-          uint64_t* d = pair_base + ((size_t)pr * kRingCap + o) * 2;
-          d[0] = (u0.op == UPD_INC || u0.op == UPD_INC_VALID) ? 1 : pick<NS>(vals, u0.slot, j);
-          d[1] = (u1.op == UPD_INC || u1.op == UPD_INC_VALID) ? 1 : pick<NS>(vals, u1.slot, j);
-        }
-      }
-      cnt += __popc(bal);
-    }
-    {  // prefetch the next tile: the loads fly while this warp works on the table
-      const int64_t nt = tile + gridDim.x;
-      if (nt < n_tiles) prefetch_tile<NS>(p, nt, vals);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // ring writes -> visible to the TMA unit
-    __syncwarp();
-    while (cnt >= 32) {
-      ring_table_phase<NS>(p, pair_base, val_base, head, 32, lane, new_groups);
-      head += 32;
-      if (head >= kRingCap) head -= kRingCap;
-      cnt -= 32;
-    }
-  }
-  __syncwarp();
-  if (cnt > 0) ring_table_phase<NS>(p, pair_base, val_base, head, cnt, lane, new_groups);
-  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) new_groups += __shfl_xor_sync(0xffffffffu, new_groups, o);
-  if (lane == 0 && new_groups) atomicAdd(p.table.n_groups, (unsigned long long)new_groups);
 }
 
 // ---------------------------------------------------------------- fused kernel (no GROUP BY)
@@ -1823,11 +1624,7 @@ __global__ void table_init_kernel(const __grid_constant__ TableDev t, const __gr
   const int64_t total = n_keys + n_slots * t.n_words;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     if (i < n_keys) t.keys[i] = kEmptyKey;
-    else {
-      const int64_t k = i - n_keys;
-      const int w = (int)(k / n_slots);
-      *word_ptr(t, k - w * n_slots, w) = init.w[w];
-    }
+    else t.states[i - n_keys] = init.w[(i - n_keys) % t.n_words];
   }
 }
 

@@ -10,7 +10,6 @@ namespace dbx {
 constexpr int kMaxSlots = 8;    // distinct input columns one kernel reads
 constexpr int kMaxUpdates = 16; // state-word updates per passing row
 constexpr int kMaxWords = 15;   // state words per group (entry = key + words)
-constexpr int kMaxPairs = 2;    // 16-byte pairs of additive state words updated by ONE TMA bulk reduction
 constexpr int kMaxComputed = DBX_MAX_COMPUTED_COLS;  // computed columns one operator evaluates
 constexpr int kMaxCompNodes = 32;                    // postfix nodes of all its computed columns together
 
@@ -110,16 +109,6 @@ struct UpdateDev {
   int32_t op;
   int32_t slot;  // input slot (unused for UPD_INC)
   int32_t word;  // state word index
-  int32_t paired; // 1: this update is carried by a pair's bulk reduction (PairDev), not by its own RED
-  int32_t ridx;   // unpaired words: index inside the slot's row-major entry (TableDev::row_base / n_single)
-  int32_t pad;
-};
-// Two additive state words of the same class (both integer adds, or both f64 adds) stored next
-// to each other (16 bytes, 16-byte aligned) and updated per row by one
-// cp.reduce.async.bulk (.add.u64 / .add.f64) of 16 bytes instead of two REDs.
-struct PairDev {
-  int32_t upd0, upd1;  // indices into upd[]: words (word0, word0 + 1 in the pair array)
-  int32_t is_f64;
   int32_t pad;
 };
 
@@ -129,18 +118,13 @@ struct PairDev {
 //                              agg_hash(key) & (n_buckets - 1), linear probing over buckets;
 //                              keys[cap] / keys[cap + 1] are 0/1 "present" flags of the two special
 //                              groups: the key equal to the EMPTY sentinel, and the NULL key;
-//   states[(cap + 2) * n_words] state word w of slot i at states[w_off[w] + i * w_stride[w]]:
-//                              paired words live in arrays of 16-byte pairs (stride 2), the others
-//                              in one array per word (stride 1) — see WordLayout in agg.cu.
+//   states[(cap + 2) * n_words] row-major: state word w of slot i at states[i * n_words + w], so the
+//                              REDs of one row fall into one or two sectors
 constexpr uint64_t kEmptyKey = 0x8000000000000000ULL;
 struct TableDev {
   uint64_t* keys;
   uint64_t* states;
   int64_t cap;
-  int64_t w_off[kMaxWords];
-  int64_t row_base;                // unpaired words: entry of slot i at states[row_base + i * n_single ...]
-  int32_t w_stride[kMaxWords];
-  int32_t n_single;
   int32_t n_words;
   int32_t probe_limit;             // buckets examined before a row is sent to the overflow list
   int32_t key_words;               // 1: 64-bit keys, buckets of 4; 2: 128-bit packed keys (HashMethodKeysU128,
@@ -156,7 +140,7 @@ struct TableDev {
 };
 
 __host__ __device__ __forceinline__ uint64_t* word_ptr(const TableDev& t, int64_t slot, int w) {
-  return t.states + t.w_off[w] + slot * t.w_stride[w];
+  return t.states + slot * t.n_words + w;
 }
 
 // Multi-column GROUP BY packed into one 64-bit key (the reference's HashMethodKeysU64 idea,
@@ -184,7 +168,6 @@ struct AggKernelParams {
   DevCol cols[kMaxSlots];
   PredNodeDev nodes[DBX_MAX_PRED_NODES];
   UpdateDev upd[kMaxUpdates];
-  PairDev pairs[kMaxPairs];
   KeyPartDev key_parts[DBX_MAX_GROUP_COLS];
   TableDev table;
   int64_t n_rows;
@@ -196,13 +179,7 @@ struct AggKernelParams {
   int32_t n_key_parts;  // > 1: the key is packed from key_parts[] (key_slot is unused)
   int32_t key_is_float; // 1: the (single) key is a float column: every NaN is one group (group_hash.rs:599-619)
   uint32_t row_base;    // added to in-launch row numbers when recording overflow rows
-  int32_t n_pairs;      // > 0: paired words go through TMA bulk reductions
-  uint32_t bulk_lanes;  // lanes (bit mask) that use the bulk path; the others use REDs for the paired words too
   int32_t debug_flags;  // perf bisecting only (env DBX_AGG_DEBUG): 1 = skip state updates, 2 = skip table probe
-  // ring kernel (filter_group_agg_ring_kernel): which input slots the table phase still needs after
-  // the predicate (key parts + arguments of unpaired updates) and where they are stored in the ring
-  int32_t ring_nsv;                 // number of stored slot arrays
-  int8_t ring_sidx[kMaxSlots];      // slot -> storage index, -1: not stored
   int32_t hot_cache;                // 1: per-CTA shared-memory cache of hot groups (skewed keys), flushed at kernel end
   // computed columns (kept behind every field above, so plans without them see the same layout):
   // comp[0, comp_pred) feed the predicate and are evaluated before it, comp[comp_pred, n_comp) after it
@@ -219,7 +196,7 @@ struct AggKernelParams {
 // build (agg_jit.cu) emits `__device__ constexpr StaticPlan jit_plan = {...}` from the operator's
 // plan, and agg_kernels.cuh reads `jit_plan.f` where the precompiled kernels read `p.f`.
 struct StaticPlan {
-  int32_t n_nodes, n_updates, key_slot, key_is_float, n_key_parts, debug_flags, n_single, hot_cache;
+  int32_t n_nodes, n_updates, key_slot, key_is_float, n_key_parts, debug_flags, n_words, hot_cache;
   PredNodeDev nodes[DBX_MAX_PRED_NODES];
   UpdateDev upd[kMaxUpdates];
   KeyPartDev key_parts[DBX_MAX_GROUP_COLS];

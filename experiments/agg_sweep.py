@@ -1,7 +1,7 @@
 """Sweeps the tuning knobs of the fused filter->hash-agg kernel in ONE process (columns generated
-once): ring kernel lane split between the TMA bulk-reduction unit and the RED path, the plain
-RED kernel, the persisting-L2 window, grid size.  Every variant's result is compared bit for bit
-with the first one (keys, sums, counts, avgs after sorting by key).
+once): the persisting-L2 window and the bisecting modes of DBX_AGG_DEBUG.  Every variant's result
+is compared bit for bit with the first one (keys, sums, counts, avgs after sorting by key).
+The kernel launcher reads DBX_AGG_GRID once per process: compare grid sizes with one run per value.
 usage: python experiments/agg_sweep.py [rows] [n_keys] [reps] [quick]"""
 import ctypes as C
 import os
@@ -27,7 +27,7 @@ blk = DataBlock([Column.device(abi.I64, rows, bufs[0].ptr), Column.device(abi.I6
 params = AggregatorParams([0], [("sum", 1), ("count", 1), ("avg", 2)])
 filt = E.eq(E.col(1) % E.lit(3), E.lit(0))
 types = [abi.I64, abi.I64, abi.F64]
-KNOBS = ["DBX_AGG_BULK", "DBX_AGG_RING", "DBX_AGG_BULK_LANES", "DBX_AGG_L2_PERSIST", "DBX_AGG_GRID", "DBX_AGG_BULK_OLD", "DBX_AGG_DEBUG"]
+KNOBS = ["DBX_AGG_L2_PERSIST", "DBX_AGG_DEBUG"]
 ref = None
 
 
@@ -66,14 +66,7 @@ def run(name, **env):
 
 
 print(f"rows {rows} keys {n_keys} reps {reps}", flush=True)
-run("plain RED kernel (no pairs), no L2 window", DBX_AGG_L2_PERSIST=0)
-run("plain RED kernel (no pairs), L2 window")
-run("pairs layout, RED kernel (ring off)", DBX_AGG_BULK=1, DBX_AGG_RING=0)
-for lanes in ["00000000", "11111111", "49249249", "55555555", "0000FFFF", "6DB6DB6D", "000FFFFF", "77777777", "00FFFFFF", "FFFFFFFF"]:
-    run(f"ring lanes={lanes} ({bin(int(lanes,16)).count('1')}/32 on TMA)", DBX_AGG_BULK=1, DBX_AGG_BULK_LANES=lanes)
-run("ring lanes=6DB6DB6D, no L2 window", DBX_AGG_BULK=1, DBX_AGG_BULK_LANES="6DB6DB6D", DBX_AGG_L2_PERSIST=0)
-for g in [4, 16]:
-    run(f"ring lanes=6DB6DB6D grid {g}/SM", DBX_AGG_BULK=1, DBX_AGG_BULK_LANES="6DB6DB6D", DBX_AGG_GRID=g)
-run("old bulk path lanes=FFFFFFFF", DBX_AGG_BULK=1, DBX_AGG_RING=0, DBX_AGG_BULK_OLD=1, DBX_AGG_BULK_LANES="FFFFFFFF")
+run("plain RED kernel, no L2 window", DBX_AGG_L2_PERSIST=0)
+run("plain RED kernel, L2 window")
 run("plain kernel front end only (dbg 2)", DBX_AGG_DEBUG=2)
 run("plain kernel probe only (dbg 1)", DBX_AGG_DEBUG=1)

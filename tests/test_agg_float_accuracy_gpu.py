@@ -220,17 +220,17 @@ def test_one_pass_overflow_and_replay(name):
         run(name, blk.split_by_rows(100_000), blk, plan(col, expected_groups=16))
 
 
-# ---------------------------------------------------------------- 6. TMA bulk pair and ring kernel
+# ---------------------------------------------------------------- 6. two f64 columns in one plan
 @pytest.mark.parametrize("name", ["cancellation", "specials"])
-def test_bulk_pair_ring_kernel(monkeypatch, name):
-    """two f64 sums form an `.add.f64` pair (the plan is then not specialised); device-resident 8-byte columns"""
-    monkeypatch.setenv("DBX_AGG_BULK", "1")
+def test_two_f64_columns_straight_line(monkeypatch, name):
+    """sum, avg, min and max of two f64 columns next to count(*) in one specialised plan; device-resident 8-byte columns"""
+    monkeypatch.setenv("DBX_AGG_JIT", "1")
     ds = dataset(name)
     blk = DataBlock([Column.from_data(ds["k"]), Column.from_data(ds["v"]), Column.from_data(ds["x"]),
                      Column.from_data(ds["y"].astype(np.float64))])
     params = AggregatorParams([0], [("sum", 2), ("avg", 2), ("min", 2), ("max", 2), ("count", None), ("sum", 3), ("avg", 3), ("min", 3)])
-    _, (v,) = run(name + "/ring", on_device([blk]), blk, params)
-    assert v == "off (plan shape not specialised)", v
+    _, (v,) = run(name + "/two-f64", on_device([blk]), blk, params)
+    assert v.startswith("specialised"), v
 
 
 # ---------------------------------------------------------------- 7. no GROUP BY

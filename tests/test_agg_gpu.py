@@ -529,24 +529,9 @@ def test_wide_keys_do_not_cross_the_row_exchange(gpu):
     part.close()
 
 
-@pytest.mark.parametrize("lanes", [None, "FFFFFFFF", "00000000", "55555555", "0000FFFF"])
-def test_ring_kernel_lane_splits(gpu, monkeypatch, lanes):
-    """The straight-line ring kernel (device-resident 8-byte columns, whole tiles): pairs of additive
-    state words updated by TMA bulk reductions on some lanes and by REDs on the others.  Every split
-    must give the oracle's result bit for bit (incl. the sentinel-valued key and a ragged tail that
-    the generic kernel finishes)."""
-    monkeypatch.setenv("DBX_AGG_BULK", "1")  # the pair layout + ring kernel are opt-in (no gain measured)
-    if lanes is not None:
-        monkeypatch.setenv("DBX_AGG_BULK_LANES", lanes)
-    blk = config2_block(3_000_017, n_keys=70_000)
-    blk.columns[0].data[:5] = -(2**63)
-    run_both(blk, CONFIG2, V_MOD3, device_resident=True)
-
-
-def test_ring_kernel_two_pairs_and_minmax(gpu, monkeypatch):
-    """sum(v), count(*), sum(x), avg(x2), min(v), max(x) over device columns: two pairs (integer and
-    f64) go through the bulk path, min/max and the leftovers through REDs."""
-    monkeypatch.setenv("DBX_AGG_BULK", "1")
+def test_device_resident_sums_count_avg_minmax(gpu):
+    """sum(v), count(*), sum(x), avg(x2), min(v), max(x) over device columns through the straight-line
+    kernel: integer and f64 sums next to min / max words in one row-major entry."""
     rng = np.random.default_rng(3)
     n = 1_500_000
     k = rng.integers(0, 20_000, n).astype(np.int64)
@@ -561,6 +546,10 @@ def test_ring_kernel_two_pairs_and_minmax(gpu, monkeypatch):
 
 def test_default_red_layout_device_resident(gpu):
     run_both(config2_block(1_200_000, n_keys=30_000), CONFIG2, V_MOD3, device_resident=True)
+    # the sentinel-valued key in the first rows, and a ragged tail that the generic kernel finishes
+    blk = config2_block(3_000_017, n_keys=70_000)
+    blk.columns[0].data[:5] = -(2**63)
+    run_both(blk, CONFIG2, V_MOD3, device_resident=True)
 
 
 def test_full_size_query_verified(gpu):

@@ -27,7 +27,7 @@
 // multi-column GROUP BY).  Up to 64 bits the entry is the same as for one key; up to 128 bits it is
 // {k0, k1, row1, p0}: still one sector, with one inlined build column instead of two.  The kernels
 // are templated on the key width KW (words) and on PACKED (key loaded from several columns); the
-// single-key instantiations <1, false> are the code as it was before composite keys.
+// single-key instantiations <1, false> read the one key column directly.
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
@@ -78,24 +78,14 @@ struct JoinKeyPack {
   int32_t pad;
 };
 
-// Radix layout: the table is cut into n_part regions of `region` entries (both powers of two);
-// a key lives in region part_owner(key, n_part) (top hash bits) at slot hash & (region - 1)
-// (low hash bits), probing wraps inside the region.  A probe block that was hash-partitioned the
-// same way walks ONE region at a time, which then sits in L2 (and in the TLB) instead of
-// scattering single-sector reads over a table many times larger than either.
 struct JoinTableDev {
   JoinEntry* entries;  // cap entries (power of two), one per 32-byte sector
   int64_t cap;
-  int64_t region;
-  int32_t n_part;
-  int32_t pad;
 };
 template <int KW = 1>
-__device__ __forceinline__ int64_t join_home(const JoinTableDev& t, uint64_t k, int64_t* region_base, uint64_t kh = 0) {
+__device__ __forceinline__ int64_t join_home(const JoinTableDev& t, uint64_t k, uint64_t kh = 0) {
   const uint64_t h = KW == 1 ? agg_hash_u64(k) : agg_hash_wide(k, kh);
-  const int64_t part = t.n_part > 1 ? (int64_t)hash_to_part(h, t.n_part) : 0;
-  *region_base = part * t.region;
-  return (int64_t)(h & (uint64_t)(t.region - 1));
+  return (int64_t)(h & (uint64_t)(t.cap - 1));
 }
 
 // build column carried inside the table entry
@@ -125,7 +115,6 @@ struct JoinProbeParams {
   JoinColDev build_cols[kMaxJoinCols];
   int32_t n_probe_cols, n_build_cols;
   int32_t kind, pad;  // dbx_join_kind
-  int64_t row_begin;  // rows [row_begin, row_begin + n_rows) of the (partitioned) probe columns
   int64_t n_rows;
   int64_t out_cap;
   unsigned long long* cursor;  // number of matches (may exceed out_cap: then the host retries)
@@ -178,10 +167,10 @@ __device__ __forceinline__ bool load_packed_key(const JoinKeyPack& pk, int64_t r
 }
 
 template <int KW, bool PACKED>
-__global__ void join_build_kernel(const __grid_constant__ DevCol key, int64_t n_rows, int64_t row_base,
+__global__ void join_build_kernel(const __grid_constant__ DevCol key, int64_t n_rows,
                                   const __grid_constant__ JoinTableDev t, const __grid_constant__ InlineColDev i0,
                                   const __grid_constant__ InlineColDev i1, const __grid_constant__ JoinKeyPack pk) {
-  const int64_t mask = t.region - 1;
+  const int64_t mask = t.cap - 1;
   JEntry<KW>* const entries = (JEntry<KW>*)t.entries;
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
     uint64_t k, kh = 0;
@@ -191,14 +180,13 @@ __global__ void join_build_kernel(const __grid_constant__ DevCol key, int64_t n_
       if (key.validity && !bit_test(key.validity, key.vbit_off + r)) continue;
       k = load_key(key, r);
     }
-    uint64_t tag = (uint64_t)(row_base + r + 1);
+    uint64_t tag = (uint64_t)(r + 1);
     uint64_t p0 = 0, p1 = 0;
     if (i0.on) { p0 = load_raw(i0.src, i0.size, r); if (!i0.valid_bytes || i0.valid_bytes[r]) tag |= 1ULL << 62; }
     if (KW == 1 && i1.on) { p1 = load_raw(i1.src, i1.size, r); if (!i1.valid_bytes || i1.valid_bytes[r]) tag |= 1ULL << 63; }
-    int64_t rb;
-    int64_t s = join_home<KW>(t, k, &rb, kh);
+    int64_t s = join_home<KW>(t, k, kh);
     for (;;) {
-      JEntry<KW>* e = entries + rb + s;
+      JEntry<KW>* e = entries + s;
       unsigned long long old = atomicCAS((unsigned long long*)&e->row1, 0ULL, (unsigned long long)tag);
       if (old == 0ULL) { fill_entry(e, k, kh, p0, p1); break; }
       s = (s + 1) & mask;
@@ -226,12 +214,6 @@ __device__ __forceinline__ void copy_value(const JoinColDev& c, int64_t src_row,
   if (c.dst_valid) c.dst_valid[dst_row] = c.src_validity ? (uint8_t)bit_test(c.src_validity, c.src_vbit_off + src_row) : 1;
 }
 
-// probe_block + InnerHashJoinStream::next fused: one thread per probe row.
-// Per step of 256 rows a CTA (1) walks every row's probe sequence, counting its matches and
-// keeping the first matching entry in registers, (2) reserves the step's output rows with ONE
-// atomic on the global cursor (block scan of the counts; a per-warp reservation costs millions of
-// same-address atomics per block and was the bottleneck), (3) writes the first match from
-// registers and re-walks the sequence only for rows with several matches.
 __device__ __forceinline__ JoinEntry load_entry(const JoinEntry* e) {
   uint64_t pol;
   asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
@@ -266,77 +248,6 @@ __device__ __forceinline__ void emit_match(const JoinProbeParams& p, int64_t r, 
     }
   }
 }
-__global__ void __launch_bounds__(kJoinBlock) join_probe_kernel(const __grid_constant__ JoinProbeParams p) {
-  __shared__ unsigned int s_warp[kJoinBlock / 32];
-  __shared__ unsigned long long s_base;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t mask = p.table.region - 1;
-  const int64_t n_iter = (p.n_rows + (int64_t)gridDim.x * blockDim.x - 1) / ((int64_t)gridDim.x * blockDim.x);
-  for (int64_t it = 0; it < n_iter; ++it) {
-    const int64_t r = p.row_begin + it * (int64_t)gridDim.x * blockDim.x + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool in_range = r < p.row_begin + p.n_rows;
-    const bool live = in_range && !(p.key.validity && !bit_test(p.key.validity, p.key.vbit_off + r));
-    uint64_t k = 0;
-    int64_t b0 = 0, rb = 0;
-    unsigned int n_match = 0;
-    JoinEntry first;
-    first.key = first.row1 = first.p0 = first.p1 = 0;
-    if (live) {
-      k = load_key(p.key, r);
-      b0 = join_home(p.table, k, &rb);
-      int64_t b = b0;
-      for (;;) {  // an empty entry ends the probe sequence
-        const JoinEntry e = load_entry(p.table.entries + rb + b);
-        if (e.row1 == 0) break;
-        if (e.key == k) { if (n_match == 0) first = e; ++n_match; }
-        b = (b + 1) & mask;
-      }
-    }
-    // semi / anti: the probe row itself is the output, at most once (a NULL key counts as no match)
-    if (p.kind == DBX_JOIN_LEFT_SEMI) n_match = n_match ? 1u : 0u;
-    else if (p.kind == DBX_JOIN_LEFT_ANTI) n_match = (in_range && n_match == 0) ? 1u : 0u;
-    const bool outer_null_row = p.kind == DBX_JOIN_LEFT && in_range && n_match == 0;  // preserved row without a match
-    if (outer_null_row) n_match = 1;
-    // block-wide exclusive scan of the match counts -> one reservation per CTA and step
-    unsigned int incl = n_match;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int up = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += up;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned int tot = 0;
-      for (int w = 0; w < kJoinBlock / 32; ++w) { const unsigned int c = s_warp[w]; s_warp[w] = tot; tot += c; }
-      s_base = tot ? atomicAdd(p.cursor, (unsigned long long)tot) : 0ULL;
-    }
-    __syncthreads();
-    int64_t pos = (int64_t)s_base + s_warp[warp] + incl - n_match;
-    __syncthreads();
-    if (outer_null_row) {
-      if (pos < p.out_cap) {
-        for (int c = 0; c < p.n_probe_cols; ++c) copy_value(p.probe_cols[c], r, pos);
-        for (int c = 0; c < p.n_build_cols; ++c) store_value(p.build_cols[c], 0, false, pos);
-      }
-    } else if (n_match && (p.kind == DBX_JOIN_LEFT_SEMI || p.kind == DBX_JOIN_LEFT_ANTI)) {
-      if (pos < p.out_cap)
-        for (int c = 0; c < p.n_probe_cols; ++c) copy_value(p.probe_cols[c], r, pos);
-    } else if (n_match) {
-      emit_match(p, r, first, pos++);
-      if (n_match > 1) {  // duplicates of the key on the build side: walk again, skip the first
-        int64_t b = b0;
-        unsigned int seen = 0;
-        for (;;) {
-          const JoinEntry e = load_entry(p.table.entries + rb + b);
-          if (e.row1 == 0) break;
-          if (e.key == k && seen++ > 0) emit_match(p, r, e, pos++);
-          b = (b + 1) & mask;
-        }
-      }
-    }
-  }
-}
 
 // Does any key occur twice on the build side?  One thread per slot walks the rest of the slot's
 // probe sequence (short at load factor <= 0.5).  A build side without duplicates (the usual
@@ -344,60 +255,63 @@ __global__ void __launch_bounds__(kJoinBlock) join_probe_kernel(const __grid_con
 // next empty entry: one dependent L2 round trip per probe row instead of two or more.
 template <int KW>
 __global__ void join_dup_check_kernel(const __grid_constant__ JoinTableDev t, unsigned int* dup) {
-  const int64_t mask = t.region - 1;
+  const int64_t mask = t.cap - 1;
   const JEntry<KW>* const entries = (const JEntry<KW>*)t.entries;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < t.cap; i += (int64_t)gridDim.x * blockDim.x) {
     const JEntry<KW> e = entries[i];
     if (e.row1 == 0) continue;
-    const int64_t rb = i & ~mask;
     int64_t s = (i + 1) & mask;
     for (;;) {
-      const JEntry<KW> f = entries[rb + s];
+      const JEntry<KW> f = entries[s];
       if (f.row1 == 0) break;
       if (key_eq(f, e.key, key_hi(e))) { *dup = 1; break; }
       s = (s + 1) & mask;
-      if (rb + s == i) break;
+      if (s == i) break;
     }
   }
 }
 
 // probe_block + JoinStream::next fused, two probe rows per thread: both rows' entry loads are in
-// flight together (the probe is bound by dependent L2 round trips, not by bytes).  UNIQUE: the
-// build side has no duplicate keys, so a row's walk ends at its first match.
+// flight together (the probe is bound by dependent L2 round trips, not by bytes).  Per step of 512
+// rows a CTA (1) walks every row's probe sequence, counting its matches and keeping the first
+// matching entry in registers, (2) reserves the step's output rows with ONE atomic on the global
+// cursor (block scan of the counts; a per-warp reservation costs millions of same-address atomics
+// per block and was the bottleneck), (3) writes the first match from registers and re-walks the
+// sequence only for rows with several matches.  UNIQUE: the build side has no duplicate keys, so
+// a row's walk ends at its first match.
 // MARK (the build-side kinds RIGHT, RIGHT SEMI, RIGHT ANTI, FULL): every matching entry's build
 // row is marked in p.matched for the final scan.  Racing stores all write 1, so no atomics.  RIGHT
 // then emits like INNER, FULL like LEFT, RIGHT SEMI / ANTI emit nothing here.
 // KW / PACKED: key width in words and composite keys (see the top of the file); a probe row with a
-// NULL in any key column is a miss.  The PACKED instantiations ask for three resident blocks per
-// SM: without a minimum ptxas caps them near 64 registers and spills, with one it takes up to 94
+// NULL in any key column is a miss.  The PACKED instantiations, and the non-unique RF ones
+// (the two widest single-key kernels), ask for three resident blocks per SM: without a minimum ptxas caps them near 64 registers and spills, with one it takes up to 94
 // registers (two blocks per SM), and the probe is bound by latency, so occupancy counts.
 // RF (single key): the join's runtime filter tests min-max and bloom before the table walk; a
 // rejected row cannot match and takes the no-match path, which is right for every kind.  The
-// RF = false instantiations compile to the code as it was before runtime filters.
+// RF = false instantiations carry none of it.
 template <int KW, bool PACKED, bool UNIQUE, bool MARK, bool RF = false>
-__global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
+__global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 0) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
   __shared__ unsigned int s_warp[kJoinBlock / 32];
   __shared__ unsigned long long s_base;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t mask = p.table.region - 1;
+  const int64_t mask = p.table.cap - 1;
   const int64_t step = (int64_t)gridDim.x * blockDim.x * 2;
   const int64_t n_iter = (p.n_rows + step - 1) / step;
-  const int64_t row_end = p.row_begin + p.n_rows;
   const JEntry<KW>* const entries = (const JEntry<KW>*)p.table.entries;
   unsigned int rf_rej = 0;
   for (int64_t it = 0; it < n_iter; ++it) {
     int64_t r[2];
-    r[0] = p.row_begin + it * step + (int64_t)blockIdx.x * blockDim.x * 2 + threadIdx.x;
+    r[0] = it * step + (int64_t)blockIdx.x * blockDim.x * 2 + threadIdx.x;
     r[1] = r[0] + blockDim.x;
     bool in_range[2], go[2];
     uint64_t k[2] = {0, 0}, kh[2] = {0, 0};
-    int64_t b0[2] = {0, 0}, rb[2] = {0, 0}, sl[2] = {0, 0};
+    int64_t b0[2] = {0, 0}, sl[2] = {0, 0};
     unsigned int n_match[2] = {0, 0};
     JEntry<KW> first[2];
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       clear_entry(first[j]);
-      in_range[j] = r[j] < row_end;
+      in_range[j] = r[j] < p.n_rows;
       if (PACKED) go[j] = in_range[j] && load_packed_key<KW>(p.pack, r[j], k[j], kh[j]);
       else go[j] = in_range[j] && !(p.key.validity && !bit_test(p.key.validity, p.key.vbit_off + r[j]));
       if (RF && go[j]) {
@@ -406,7 +320,7 @@ __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel
       }
       if (go[j]) {
         if (!PACKED) k[j] = load_key(p.key, r[j]);
-        b0[j] = join_home<KW>(p.table, k[j], &rb[j], kh[j]);
+        b0[j] = join_home<KW>(p.table, k[j], kh[j]);
         sl[j] = b0[j];
       }
     }
@@ -414,7 +328,7 @@ __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel
       JEntry<KW> e[2];
 #pragma unroll
       for (int j = 0; j < 2; ++j)
-        if (go[j]) e[j] = load_entry(entries + rb[j] + sl[j]);
+        if (go[j]) e[j] = load_entry(entries + sl[j]);
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         if (!go[j]) continue;
@@ -477,7 +391,7 @@ __global__ void __launch_bounds__(kJoinBlock, PACKED ? 3 : 0) join_probe2_kernel
           int64_t b = b0[j];
           unsigned int seen = 0;
           for (;;) {
-            const JEntry<KW> e = load_entry(entries + rb[j] + b);
+            const JEntry<KW> e = load_entry(entries + b);
             if (e.row1 == 0) break;
             if (key_eq(e, k[j], kh[j]) && seen++ > 0) emit_match<PACKED>(p, r[j], e, pos++);
             b = (b + 1) & mask;
@@ -549,14 +463,6 @@ __global__ void __launch_bounds__(kJoinBlock) join_final_scan_kernel(const __gri
   }
 }
 
-// Pull one table region into L2 with full-line sequential reads before it is probed: the probes
-// themselves would fetch it as scattered 32-byte sectors, which HBM serves an order of magnitude
-// slower than a stream.
-__global__ void l2_prefetch_kernel(const char* base, int64_t bytes) {
-  for (int64_t off = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 128; off < bytes; off += (int64_t)gridDim.x * blockDim.x * 128)
-    asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(base + off));
-}
-
 __global__ void pack_bits_kernel(const uint8_t* bytes, int64_t n, uint8_t* bits) {
   int64_t nb = (n + 7) / 8;
   for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += (int64_t)gridDim.x * blockDim.x) {
@@ -606,13 +512,8 @@ class JoinOp : public Op {
   int64_t table_cap = 0;
   PinnedBuf host;
   int inline_col[2] = {-1, -1};
-  int n_part = 1;
-  int64_t region = 0;
-  DevBuf part_counters;
   bool build_unique = false;  // no key occurs twice on the build side (checked after the build)
-  DevBuf part_cols[kMaxJoinCols];
-  std::vector<int64_t> part_offs;
-  JoinTableDev table_view() const { return JoinTableDev{(JoinEntry*)table_buf.p, table_cap, region, n_part, 0}; }
+  JoinTableDev table_view() const { return JoinTableDev{(JoinEntry*)table_buf.p, table_cap}; }
   std::vector<std::unique_ptr<OwnedBlock>> outputs;  // joined blocks waiting to be pulled (device resident)
   size_t next_out = 0;
   DevBuf matched;             // build-side kinds: one byte per build row, 1 once any probe row matched it
@@ -743,34 +644,6 @@ class JoinOp : public Op {
   int32_t finish() override {
     table_cap = std::max<int64_t>(next_pow2_i64(2 * std::max<int64_t>(build_rows, 1)), 1024);  // with_build_row_num
     if (build_rows >= (int64_t)kRowMask) { err.set("join: too many build rows"); return DBX_ERR_UNSUPPORTED; }
-    // radix regions: cut a table that is far larger than L2 into pieces of <= 32 MB
-    n_part = 1;
-    {
-      const int64_t bytes = table_cap * (int64_t)sizeof(JoinEntry);
-      // Radix regions are OFF by default: once the probe stops at its first match (unique build
-      // keys) one random HBM sector per row costs less than the extra partition pass over the
-      // probe block.  DBX_JOIN_REGION_BYTES=<bytes> turns them on (tests exercise both).
-      // Composite keys stay in one region: hash_partition_device partitions by one column.
-      int64_t target = 0;
-      if (const char* e = getenv("DBX_JOIN_REGION_BYTES")) target = atoll(e);
-      if (!packed && target > 0 && bytes > 3 * target) {
-        while (n_part < kMaxParts && bytes / n_part > target) n_part *= 2;
-      }
-    }
-    region = table_cap / n_part;
-    DBX_CUDA_TRY(err, part_counters.ensure((size_t)kMaxParts * 8));
-    if (n_part > 1) {  // a skewed key distribution could overfill a region: then fall back to one region
-      PartParams cp;
-      memset(&cp, 0, sizeof(cp));
-      cp.key.data = build[prm.build_key_col].data.p;
-      cp.key.dtype = build_dtype[prm.build_key_col];
-      cp.n_cols = 0; cp.n_parts = n_part; cp.n_rows = build_rows;
-      std::vector<int64_t> offs((size_t)n_part + 1);
-      DBX_TRY(hash_partition_device(err, stream, cp, (unsigned long long*)part_counters.p, offs.data()));
-      int64_t worst = 0;
-      for (int i = 0; i < n_part; ++i) worst = std::max(worst, offs[i + 1] - offs[i]);
-      if (worst * 10 > region * 7) { n_part = 1; region = table_cap; }
-    }
     DBX_CUDA_TRY(err, table_buf.ensure((size_t)table_cap * sizeof(JoinEntry)));
     DBX_CUDA_TRY(err, cudaMemsetAsync(table_buf.p, 0, (size_t)table_cap * sizeof(JoinEntry), stream));
     if (build_side_kind(prm.kind)) {  // the matched map, indexed by build row (NULL-key rows stay 0)
@@ -826,9 +699,9 @@ class JoinOp : public Op {
         ++k;
       }
       const int grid = grid_rows(build_rows);
-      if (!packed) join_build_kernel<1, false><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1], pk);
-      else if (key_words == 1) join_build_kernel<1, true><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1], pk);
-      else join_build_kernel<2, true><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, 0, t, ic[0], ic[1], pk);
+      if (!packed) join_build_kernel<1, false><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, t, ic[0], ic[1], pk);
+      else if (key_words == 1) join_build_kernel<1, true><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, t, ic[0], ic[1], pk);
+      else join_build_kernel<2, true><<<grid, kJoinBlock, 0, stream>>>(key, build_rows, t, ic[0], ic[1], pk);
       count_launch();
       DBX_CUDA_TRY(err, cudaGetLastError());
       DBX_CUDA_TRY(err, cudaMemsetAsync(cursor.p, 0, 16, stream));
@@ -856,17 +729,13 @@ class JoinOp : public Op {
     }
   }
   void launch_probe(const JoinProbeParams& pp, int64_t rows) {
-    static const bool old_probe = getenv("DBX_JOIN_OLD_PROBE") != nullptr;
     const int grid = grid_rows((rows + 1) / 2);
-    // DBX_JOIN_OLD_PROBE is an ablation of the single-key probe-side kinds; the build-side kinds and
-    // composite keys always take the two-row kernel
     if (packed) {
       if (key_words == 2) launch_probe2<2, true>(pp, grid);
       else launch_probe2<1, true>(pp, grid);
       return;
     }
     if (rf_probe) { launch_probe2<1, false, true>(pp, grid); return; }
-    if (old_probe && !pp.matched) { join_probe_kernel<<<grid_rows(rows), kJoinBlock, 0, stream>>>(pp); return; }
     launch_probe2<1, false>(pp, grid);
   }
 
@@ -889,23 +758,6 @@ class JoinOp : public Op {
     const bool marks_only = prm.kind == DBX_JOIN_RIGHT_SEMI || prm.kind == DBX_JOIN_RIGHT_ANTI;
     int64_t out_cap = marks_only ? 0 : n + n / 8 + 1024;  // optimistic: about one match per probe row
     DBX_TRY(timing_begin());
-    // radix probe: reorder the block region by region (row order of a join result is unspecified)
-    bool can_part = n_part > 1 && (n >= (1 << 16) || getenv("DBX_JOIN_REGION_BYTES"));
-    for (int c = 0; c < n_probe_cols && can_part; ++c) can_part = !cols[c].validity;
-    if (can_part) {
-      PartParams pq;
-      memset(&pq, 0, sizeof(pq));
-      pq.key = cols[prm.probe_key_col];
-      pq.n_cols = n_probe_cols; pq.n_parts = n_part; pq.n_rows = n;
-      for (int c = 0; c < n_probe_cols; ++c) {
-        const int sz = dtype_size(probe_dtype[c]);
-        DBX_CUDA_TRY(err, part_cols[c].ensure((size_t)n * sz));
-        pq.cols[c].src = cols[c].data; pq.cols[c].dst = part_cols[c].p; pq.cols[c].size = sz;
-      }
-      part_offs.assign((size_t)n_part + 1, 0);
-      DBX_TRY(hash_partition_device(err, stream, pq, (unsigned long long*)part_counters.p, part_offs.data()));
-      for (int c = 0; c < n_probe_cols; ++c) cols[c].data = part_cols[c].p;
-    }
     for (int attempt = 0; attempt < 2; ++attempt) {
       auto ob = std::make_unique<OwnedBlock>();
     ob->stream = stream;  // freed in order behind this operator's enqueued work
@@ -975,22 +827,8 @@ class JoinOp : public Op {
         DBX_TRY(add_out(pp.build_cols[c], build_dtype[c], build_nullable[c] || prm.kind == DBX_JOIN_LEFT || prm.kind == DBX_JOIN_FULL));
       }
       DBX_CUDA_TRY(err, cudaMemsetAsync(cursor.p, 0, 8, stream));
-      if (can_part) {  // region by region: stream the region into L2, then probe the rows that hash into it
-        for (int part = 0; part < n_part; ++part) {
-          const int64_t m = part_offs[part + 1] - part_offs[part];
-          if (m == 0) continue;
-          const int64_t bytes = region * (int64_t)sizeof(JoinEntry);
-          l2_prefetch_kernel<<<(int)std::min<int64_t>((bytes / 128 + 255) / 256, (int64_t)kNumSMs * 8), 256, 0, stream>>>(
-              (const char*)table_buf.p + (int64_t)part * bytes, bytes);
-          pp.row_begin = part_offs[part];
-          pp.n_rows = m;
-          launch_probe(pp, m);
-          count_launch(2);
-        }
-      } else {
-        launch_probe(pp, n);
-        count_launch();
-      }
+      launch_probe(pp, n);
+      count_launch();
       DBX_CUDA_TRY(err, cudaGetLastError());
       DBX_CUDA_TRY(err, cudaMemcpyAsync(host.p, cursor.p, 8, cudaMemcpyDeviceToHost, stream));
       DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));

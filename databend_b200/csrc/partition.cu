@@ -121,9 +121,8 @@ __global__ void __launch_bounds__(256) partition_scatter_kernel(const __grid_con
 }  // namespace
 
 
-// Stream-ordered hash partition of device columns (used by dbx_hash_partition and by the radix
-// probe of the join).  `counters`: device scratch of kMaxParts u64.  host_counts/host_offsets:
-// host arrays; the call synchronises the stream once (the counts are needed to place the runs).
+// Stream-ordered hash partition of device columns (used by dbx_hash_partition).  `counters`:
+// device scratch of kMaxParts u64.  host_counts/host_offsets: host arrays; the call synchronises the stream once (the counts are needed to place the runs).
 int32_t hash_partition_device(ErrorSink& err, cudaStream_t stream, const PartParams& params, unsigned long long* counters,
                               int64_t* host_offsets) {
   PartParams p = params;

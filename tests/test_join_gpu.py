@@ -116,11 +116,10 @@ def test_wide_build_side_inline_and_gather(gpu):
     run_join(build, probe, 2, 0, build_split=1500, probe_split=2500)
 
 
-def test_radix_partitioned_probe(gpu, monkeypatch):
-    """Force the radix layout (table cut into regions, probe block partitioned the same way) at
-    test size: same multiset of joined rows, incl. duplicate build keys, misses and a skewed build
-    side that must fall back to a single region."""
-    monkeypatch.setenv("DBX_JOIN_REGION_BYTES", str(64 << 10))
+def test_duplicate_build_keys_misses_and_one_long_chain(gpu):
+    """Duplicate build keys with misses on both sides, over a probe split into blocks and over a
+    device-resident probe block; then a build side whose keys are all equal, so that one probe
+    sequence is as long as the build side and every matching probe row emits all of it."""
     rng = np.random.default_rng(31)
     nb, npb = 60_000, 200_000
     build = DataBlock([Column.from_data(rng.integers(0, 50_000, nb).astype(np.int64)), Column.from_data(rng.integers(-9, 9, nb).astype(np.int64)),
@@ -134,7 +133,7 @@ def test_radix_partitioned_probe(gpu, monkeypatch):
 
 
 @pytest.mark.parametrize("kind_name", ["semi", "anti"])
-def test_left_semi_and_anti(gpu, kind_name, monkeypatch):
+def test_left_semi_and_anti(gpu, kind_name):
     """LEFT SEMI / LEFT ANTI (left_join_semi.rs, left_join_anti.rs): probe rows with at least one /
     with no match, probe columns only, each row at most once; a NULL probe key never matches."""
     rng = np.random.default_rng(41)
@@ -148,28 +147,25 @@ def test_left_semi_and_anti(gpu, kind_name, monkeypatch):
     matched[pi] = True
     expect = np.nonzero(matched if kind_name == "semi" else ~matched)[0]
     kind = abi.JOIN_LEFT_SEMI if kind_name == "semi" else abi.JOIN_LEFT_ANTI
-    for radix in (False, True):
-        if radix:
-            monkeypatch.setenv("DBX_JOIN_REGION_BYTES", str(64 << 10))
-        j = HashJoin(schema_types(build), schema_types(probe), 0, 0, kind=kind)
-        j.add_block(build)
-        j.final_build()
-        outs = []
-        for p in probe.split_by_rows(17_000):
-            outs.extend(j.probe_block(p))
-        j.close()
-        assert all(o.num_columns() == 2 for o in outs)
-        tags = np.sort(np.concatenate([o.columns[1].values() for o in outs])) if outs else np.empty(0, np.int64)
-        np.testing.assert_array_equal(tags, expect)
-        keys = np.concatenate([o.columns[0].values() for o in outs])
-        kval = np.concatenate([o.columns[0].valid_mask() for o in outs])
-        order = np.argsort(np.concatenate([o.columns[1].values() for o in outs]))
-        np.testing.assert_array_equal(kval[order], probe.columns[0].valid_mask()[expect])
-        m = kval[order]
-        np.testing.assert_array_equal(keys[order][m], probe.columns[0].values()[expect][m])
+    j = HashJoin(schema_types(build), schema_types(probe), 0, 0, kind=kind)
+    j.add_block(build)
+    j.final_build()
+    outs = []
+    for p in probe.split_by_rows(17_000):
+        outs.extend(j.probe_block(p))
+    j.close()
+    assert all(o.num_columns() == 2 for o in outs)
+    tags = np.sort(np.concatenate([o.columns[1].values() for o in outs])) if outs else np.empty(0, np.int64)
+    np.testing.assert_array_equal(tags, expect)
+    keys = np.concatenate([o.columns[0].values() for o in outs])
+    kval = np.concatenate([o.columns[0].valid_mask() for o in outs])
+    order = np.argsort(np.concatenate([o.columns[1].values() for o in outs]))
+    np.testing.assert_array_equal(kval[order], probe.columns[0].valid_mask()[expect])
+    m = kval[order]
+    np.testing.assert_array_equal(keys[order][m], probe.columns[0].values()[expect][m])
 
 
-def test_left_outer(gpu, monkeypatch):
+def test_left_outer(gpu):
     """LEFT join (left_join.rs): every probe row; rows without a match carry NULL in all build
     columns (which come back Nullable).  Compared as a multiset with rows derived from the oracle's
     inner pairs plus the unmatched probe rows."""
@@ -193,23 +189,20 @@ def test_left_outer(gpu, monkeypatch):
         vals = np.concatenate([c.values()[bi], np.zeros(len(un), dtype=c.values().dtype)])
         valid = np.concatenate([c.valid_mask()[bi], np.zeros(len(un), dtype=bool)])
         exp_cols.append(Column.from_data(vals, c.dtype, validity=valid))
-    for radix in (False, True):
-        if radix:
-            monkeypatch.setenv("DBX_JOIN_REGION_BYTES", str(64 << 10))
-        j = HashJoin(schema_types(build), schema_types(probe), 0, 0, kind=abi.JOIN_LEFT)
-        j.add_block(build)
-        j.final_build()
-        outs = []
-        for p in probe.split_by_rows(11_000):
-            outs.extend(j.probe_block(p))
-        j.close()
-        assert sum(o.num_rows for o in outs) == len(pi) + len(un)
-        got_cols = []
-        for ci in range(6):
-            vals = np.concatenate([o.columns[ci].values() for o in outs])
-            valid = np.concatenate([o.columns[ci].valid_mask() for o in outs])
-            got_cols.append(Column.from_data(vals, outs[0].columns[ci].dtype, validity=valid))
-        np.testing.assert_array_equal(joined_rows_sorted(got_cols), joined_rows_sorted(exp_cols))
+    j = HashJoin(schema_types(build), schema_types(probe), 0, 0, kind=abi.JOIN_LEFT)
+    j.add_block(build)
+    j.final_build()
+    outs = []
+    for p in probe.split_by_rows(11_000):
+        outs.extend(j.probe_block(p))
+    j.close()
+    assert sum(o.num_rows for o in outs) == len(pi) + len(un)
+    got_cols = []
+    for ci in range(6):
+        vals = np.concatenate([o.columns[ci].values() for o in outs])
+        valid = np.concatenate([o.columns[ci].valid_mask() for o in outs])
+        got_cols.append(Column.from_data(vals, outs[0].columns[ci].dtype, validity=valid))
+    np.testing.assert_array_equal(joined_rows_sorted(got_cols), joined_rows_sorted(exp_cols))
 
 
 def test_mixed_width_keys_and_signed_vs_uint64_refused(gpu):

@@ -236,9 +236,9 @@ def test_refusals(gpu):
 
 
 @pytest.mark.parametrize("layout", ["2xI32", "2xI64"])
-def test_region_bytes_leave_composite_keys_in_one_region(gpu, layout, monkeypatch):
+def test_larger_unique_build_side_over_a_split_probe(gpu, layout):
+    """The packed kernels at 60 000 x 200 000 rows with the probe side in 70 000-row blocks."""
     build, probe, bk, pk = tables(layout, 31, nb=60_000, npr=200_000, unique=True)
-    monkeypatch.setenv("DBX_JOIN_REGION_BYTES", str(64 << 10))
     for kind in ("inner", "left", "right", "full"):
         run_and_compare(kind, build, probe, bk, pk, probe_split=70_000)
 

@@ -129,17 +129,16 @@ def test_random_nullable_duplicates_and_misses(gpu, kind, monkeypatch):
 
 
 @pytest.mark.parametrize("kind", list(KINDS))
-def test_unique_build_side_radix_regions(gpu, kind, monkeypatch):
-    """Unique build keys (the early-stop probe) with radix regions on and off, and a build side
-    with duplicates under radix regions; device-resident probe blocks."""
+def test_unique_and_duplicate_build_sides_over_split_probes(gpu, kind):
+    """Unique build keys (the early-stop probe) at 60 000 x 200 000 rows, over a probe split into
+    blocks and over a device-resident probe block; then a build side of the same size with
+    duplicate and NULL keys."""
     rng = np.random.default_rng(19)
     nb, npr = 60_000, 200_000
     dk = rng.permutation(nb).astype(np.int64) * 7 - 1000
     build = DataBlock([Column.from_data(dk), Column.from_data(rng.integers(-9, 9, nb).astype(np.int64))])
     probe = DataBlock([Column.from_data(np.concatenate([dk[rng.integers(0, nb * 8 // 10, npr - 5000)], rng.integers(10**9, 2 * 10**9, 5000)])),
                        Column.from_data(rng.integers(0, 2**31, npr).astype(np.int32))])
-    run_and_compare(kind, build, probe, 0, 0, probe_split=70_000)
-    monkeypatch.setenv("DBX_JOIN_REGION_BYTES", str(64 << 10))
     run_and_compare(kind, build, probe, 0, 0, probe_split=70_000)
     run_and_compare(kind, build, probe, 0, 0, device_resident=True)
     dup, p2 = random_tables(29, nb=60_000, npr=100_000, key_range=40_000)

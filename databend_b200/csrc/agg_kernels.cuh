@@ -1119,7 +1119,7 @@ __device__ __forceinline__ void filter_partition_ring_body(const AggKernelParams
 // buckets) held in shared memory: the slice's keys and state words are loaded from the table, the
 // partition's rows are streamed from pass 1's buffers, every row is probed in the slice in the same
 // linear bucket order as find_or_insert_slow and updates its group with shared-memory atomics
-// (slice_update), and the slice is stored back with plain stores (no other CTA touches it).  A row is
+// (slice_update_words), and the slice is stored back with plain stores (no other CTA touches it).  A row is
 // deferred to a list, which the fused kernel then runs against the whole table, when its probe
 // would leave the slice (this includes the wrap from the last bucket to bucket 0), when it reaches
 // probe_limit (or kSliceProbes), or when its key is the EMPTY pattern: these are the only rows this
@@ -1132,31 +1132,39 @@ __device__ __forceinline__ void filter_partition_ring_body(const AggKernelParams
 // kernel reads them directly.
 //
 // The cost of a row is a chain of shared-memory accesses (bucket loads, then atomics whose returned
-// values feed the next step), so what matters is how many rows are in flight per SM.  The partition's
-// rows are therefore copied into shared memory with cp.async in stages of slice_stage_rows<NS>() rows,
-// double-buffered (the next stage is in flight while this one is aggregated), and no row values are
-// held in registers across a stage: kSliceBlock = 1024 threads (32 warps per SM, at most 64 registers)
-// work on a stage.  Each thread takes RPT rows of it and handles them in phases: it loads the first
-// bucket of every row (two 128-bit shared loads each) before it resolves any slot, then issues the
-// updates of all of them update by update, so the atomics of different rows are in flight together.
+// values feed the next step), so what matters is how many rows are in flight per SM, and that no warp
+// waits for another.  kSliceBlock = 1024 threads (32 warps per SM, at most 64 registers) each stream
+// their own rows: the partition is cut into blocks of slice_warp_rows<NS>() rows (32 x RPT), block b
+// belongs to warp b mod 32, and each warp copies its blocks into its own kSliceRing buffers in shared
+// memory with cp.async (the next block is in flight while this one is aggregated), synchronised with
+// __syncwarp only.  So a warp slowed by a long probe, a compare-and-swap retry or a deferred-row
+// reservation holds back no other warp, and the CTA meets at a barrier only after the slice is loaded
+// and before it is stored back.  No row values are held in registers across a block.  Each thread
+// handles its RPT rows in phases: it loads the first bucket of every row (two 128-bit shared loads
+// each) before it resolves any slot, then issues the updates of all rows and all state words phase by
+// phase (slice_update_words), so that independent atomics are in flight together.
 constexpr int kSliceBlock = 1024;
+constexpr int kSliceWarps = kSliceBlock / 32;
+constexpr int kSliceRing = 2;  // row buffers per warp
 constexpr int kSliceFillNum = 3, kSliceFillDen = 4;
 // Buckets a row probes in its slice before it is deferred.  Below the load-factor budget chains this
 // long are rare; a slice that fills up (more groups than the table was sized for) defers its rows after
 // a few probes instead of walking every full bucket to the slice's end.
 constexpr int kSliceProbes = 8;
 constexpr size_t kSliceBytes = 128 << 10;       // shared memory for one slice: keys + state words
-constexpr size_t kSliceStageBytes = 96 << 10;   // both row buffers: a full slice and its rows take 224 of the 227 KB a CTA may use
-// rows per stage: a power of two from kSliceBlock / 2 to 2 * kSliceBlock (more rows per thread spill at 64
-// registers), two buffers of NS slots within kSliceStageBytes
+constexpr size_t kSliceStageBytes = 96 << 10;   // every warp's row buffers: a full slice and its rows take 224 of the 227 KB a CTA may use
+// Rows of one per-warp block: 64 (two per lane) or 32 where kSliceRing buffers of NS slots for each of the
+// 32 warps fit kSliceStageBytes (more rows per thread spill at 64 registers); NS = 7 and 8 only fit 24
+// (lanes 24..31 idle, so 768 rows of the CTA are in flight).  A multiple of 8, so every buffer and every
+// block's first row stays 16-byte aligned for cp.async.
 template <int NS>
-__host__ __device__ constexpr int slice_stage_rows() {
-  int r = 2 * kSliceBlock;
-  while (r > kSliceBlock / 2 && (size_t)2 * NS * 8 * r > kSliceStageBytes) r >>= 1;
+__host__ __device__ constexpr int slice_warp_rows() {
+  int r = 64;
+  while (r > 8 && (size_t)kSliceWarps * kSliceRing * NS * 8 * r > kSliceStageBytes) r -= r > 32 ? 32 : 8;
   return r;
 }
 template <int NS>
-__host__ __device__ constexpr size_t slice_stage_bytes() { return (size_t)2 * NS * 8 * slice_stage_rows<NS>(); }
+__host__ __device__ constexpr size_t slice_stage_bytes() { return (size_t)kSliceWarps * kSliceRing * NS * 8 * slice_warp_rows<NS>(); }
 struct SliceIn {
   const uint64_t* in[kMaxSlots];  // pass 1's partitions: per slot [P][cap_p]
   const unsigned long long* counts;
@@ -1169,15 +1177,16 @@ struct SliceIn {
 __device__ __forceinline__ void cp_async_16(void* smem, const void* gmem) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
 }
-// Rows [r0, r0 + min(B, n - r0)) of the partition at `base`, every slot, into buf[NS][B] as one cp.async
-// group.  The copy moves whole 16-byte pairs of rows: a partition's buffer holds cap_p >= n rows and cap_p
-// is a multiple of 4, so the pair that holds the last row stays inside it (its other row is not used).
-template <int NS, int B>
-__device__ __forceinline__ void slice_stage_copy(const SliceIn& si, int64_t base, int64_t r0, int64_t n, uint64_t* buf) {
-  const int pairs = (int)((min((int64_t)B, n - r0) + 1) >> 1);
+// Rows [r0, r0 + min(WR, n - r0)) of the partition at `base`, every slot, into buf[NS][WR] as one cp.async
+// group of the calling warp (every lane commits one, so the lanes' group counts agree).  The copy moves
+// whole 16-byte pairs of rows: a partition's buffer holds cap_p >= n rows and cap_p is a multiple of 4,
+// so the pair that holds the last row stays inside it (its other row is not used).
+template <int NS, int WR>
+__device__ __forceinline__ void slice_warp_copy(const SliceIn& si, int64_t base, int64_t r0, int64_t n, uint64_t* buf, int lane) {
+  const int pairs = (int)((min((int64_t)WR, n - r0) + 1) >> 1);
 #pragma unroll
   for (int s = 0; s < NS; ++s)
-    for (int c = threadIdx.x; c < pairs; c += kSliceBlock) cp_async_16(buf + (size_t)s * B + 2 * c, si.in[s] + base + r0 + 2 * c);
+    for (int c = lane; c < pairs; c += 32) cp_async_16(buf + (size_t)s * WR + 2 * c, si.in[s] + base + r0 + 2 * c);
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
@@ -1228,52 +1237,91 @@ __device__ __noinline__ int64_t slice_probe(uint64_t* skeys, uint64_t key, int64
   }
 }
 
-// One state word of each of a thread's RPT rows (w[r]: the word; bit r of `on`: row r has a slot here).
-// Integer adds are two native 32-bit shared adds plus a carry, as in smem_add_u64, with the low halves of
-// all rows issued before any carry is looked at; the compare-and-swap loops of f64 sums run side by side;
-// minima and maxima use hot_update's shared-memory atomics.
-template <int RPT>
-__device__ __forceinline__ void slice_update(int op, uint64_t* const (&w)[RPT], const uint64_t (&v)[RPT], uint32_t on) {
-  if (op == UPD_INC || op == UPD_INC_VALID || op == UPD_ADD_INT) {
-    unsigned int old[RPT];
+// (state word, row) pairs per call of slice_update_words: the specialised build takes every word of its
+// plan at once (the plan is a constant, so the phases unroll to straight-line code); the precompiled one
+// reads the plan at run time and takes a few words at a time, so that what the first phase returns fits
+// its registers.
+#ifdef DBX_JIT
+constexpr int kSliceUpdPairs = 32;
+#else
+constexpr int kSliceUpdPairs = 4;
+#endif
+
+// Update words upd[u0, u0 + G) of a thread's RPT rows (row r is lane + 32 r of the warp's block `st`; bit r
+// of `on`: it has slot slot[r]), phase by phase over all rows and words, so that no shared-memory access
+// waits on a result it does not need:
+//  1. the low halves of the integer words (counts and integer sums are two native 32-bit shared adds plus
+//     a carry, as in smem_add_u64) and the first load of every f64 sum;
+//  2. the high halves with their carries, the first compare-and-swap of every f64 sum, and the minima and
+//     maxima (hot_update's shared-memory atomics);
+//  3. one retry loop over the (row, f64 word) pairs whose compare-and-swap lost a race.
+template <int RPT, int G, int WR>
+__device__ __forceinline__ void slice_update_words(const AggKernelParams& p, int u0, const uint64_t* st, int lane, uint64_t* sst, int nw,
+                                                   const int (&slot)[RPT], uint32_t on) {
+  static_assert(G * RPT <= 32, "one pending bit per (word, row)");
+  auto word = [&](int u, int r) { return sst + slot[r] * nw + PLN(upd[u]).word; };
+  auto val = [&](int u, int r) { return st[PLN(upd[u]).slot * WR + lane + 32 * r]; };
+  auto is_int = [](int op) { return op == UPD_INC || op == UPD_INC_VALID || op == UPD_ADD_INT; };
+  uint64_t got[G][RPT];  // what phase 1 returned: the old low half of an integer word, the f64 word
 #pragma unroll
-    for (int r = 0; r < RPT; ++r)
-      if ((on >> r) & 1) old[r] = atomicAdd(reinterpret_cast<unsigned int*>(w[r]), op == UPD_ADD_INT ? (unsigned int)v[r] : 1u);
+  for (int g = 0; g < G; ++g) {
+    const int u = u0 + g;
+    if (u >= PLN(n_updates)) break;
+    const int op = PLN(upd[u]).op;
 #pragma unroll
     for (int r = 0; r < RPT; ++r) {
       if (!((on >> r) & 1)) continue;
-      const unsigned int lo = op == UPD_ADD_INT ? (unsigned int)v[r] : 1u, hi = op == UPD_ADD_INT ? (unsigned int)(v[r] >> 32) : 0u;
-      const unsigned int up = hi + (old[r] + lo < old[r] ? 1u : 0u);
-      if (up) atomicAdd(reinterpret_cast<unsigned int*>(w[r]) + 1, up);
+      if (is_int(op)) got[g][r] = atomicAdd(reinterpret_cast<unsigned int*>(word(u, r)), op == UPD_ADD_INT ? (unsigned int)val(u, r) : 1u);
+      else if (op == UPD_ADD_F64) got[g][r] = *reinterpret_cast<volatile unsigned long long*>(word(u, r));
     }
-    return;
   }
-  if (op == UPD_ADD_F64) {
-    unsigned long long cur[RPT];
+  uint32_t pend = 0;  // bit g * RPT + r: row r's compare-and-swap of word u0 + g lost a race
 #pragma unroll
-    for (int r = 0; r < RPT; ++r)
-      if ((on >> r) & 1) cur[r] = *reinterpret_cast<volatile unsigned long long*>(w[r]);
-    for (uint32_t pend = on; pend;) {
+  for (int g = 0; g < G; ++g) {
+    const int u = u0 + g;
+    if (u >= PLN(n_updates)) break;
+    const int op = PLN(upd[u]).op;
 #pragma unroll
-      for (int r = 0; r < RPT; ++r) {
-        if (!((pend >> r) & 1)) continue;
-        const unsigned long long nv = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur[r]) + __longlong_as_double((long long)v[r]));
-        const unsigned long long o = atomicCAS(reinterpret_cast<unsigned long long*>(w[r]), cur[r], nv);
-        if (o == cur[r]) pend &= ~(1u << r);
-        cur[r] = o;
+    for (int r = 0; r < RPT; ++r) {
+      if (!((on >> r) & 1)) continue;
+      const uint64_t v = op == UPD_INC || op == UPD_INC_VALID ? 1 : val(u, r);
+      if (is_int(op)) {
+        const unsigned int old = (unsigned int)got[g][r], lo = (unsigned int)v, up = (unsigned int)(v >> 32) + (old + lo < old ? 1u : 0u);
+        if (up) atomicAdd(reinterpret_cast<unsigned int*>(word(u, r)) + 1, up);
+      } else if (op == UPD_ADD_F64) {
+        const unsigned long long cur = got[g][r];
+        const unsigned long long nv = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur) + __longlong_as_double((long long)v));
+        const unsigned long long o = atomicCAS(reinterpret_cast<unsigned long long*>(word(u, r)), cur, nv);
+        if (o != cur) pend |= 1u << (g * RPT + r);
+        got[g][r] = o;
+      } else {
+        hot_update(op, word(u, r), v, true);
       }
     }
-    return;
   }
+  while (pend) {
 #pragma unroll
-  for (int r = 0; r < RPT; ++r)
-    if ((on >> r) & 1) hot_update(op, w[r], v[r], true);
+    for (int g = 0; g < G; ++g) {
+      const int u = u0 + g;
+      if (u >= PLN(n_updates)) break;
+      if (PLN(upd[u]).op != UPD_ADD_F64) continue;
+#pragma unroll
+      for (int r = 0; r < RPT; ++r) {
+        if (!((pend >> (g * RPT + r)) & 1)) continue;
+        const unsigned long long cur = got[g][r];
+        const unsigned long long nv = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur) + __longlong_as_double((long long)val(u, r)));
+        const unsigned long long o = atomicCAS(reinterpret_cast<unsigned long long*>(word(u, r)), cur, nv);
+        if (o == cur) pend &= ~(1u << (g * RPT + r));
+        got[g][r] = o;
+      }
+    }
+  }
 }
 
 template <int NS>
 __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const SliceIn& si) {
-  constexpr int B = slice_stage_rows<NS>();
-  constexpr int RPT = B >= kSliceBlock ? B / kSliceBlock : 1;
+  constexpr int WR = slice_warp_rows<NS>();
+  constexpr int RPT = (WR + 31) / 32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ unsigned int s_fill, s_fill0;  // occupied slots of the slice: now, and when it was loaded
   const TableDev& t = p.table;
@@ -1282,12 +1330,16 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
   const int64_t S = si.slice_slots;
   uint64_t* skeys = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t* sst = skeys + S;                 // state word w of slot i at sst[i * nw + w]
-  uint64_t* stage = sst + S * nw;            // two buffers of [NS][B] row values
+  uint64_t* stage = sst + S * nw;            // per warp, kSliceRing buffers of [NS][WR] row values
   const int64_t slot0 = (int64_t)blockIdx.x * S;
   const int64_t n = (int64_t)si.counts[blockIdx.x];
   const int64_t base = (int64_t)blockIdx.x * si.cap_p;
-  const int64_t n_stages = (n + B - 1) / B;
-  if (n_stages > 0) slice_stage_copy<NS, B>(si, base, 0, n, stage);  // in flight while the slice is loaded
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint64_t* ring = stage + (size_t)warp * kSliceRing * NS * WR;
+  // block b of the partition (rows [b * WR, b * WR + WR)) belongs to warp b mod kSliceWarps
+  const int64_t n_blocks = (n + WR - 1) / WR;
+  const int my_blocks = warp < n_blocks ? (int)((n_blocks - 1 - warp) / kSliceWarps) + 1 : 0;
+  if (my_blocks > 0) slice_warp_copy<NS, WR>(si, base, (int64_t)warp * WR, n, ring, lane);  // in flight while the slice is loaded
   if (threadIdx.x == 0) s_fill = s_fill0 = 0;
   __syncthreads();
   ulonglong2* gkeys = reinterpret_cast<ulonglong2*>(t.keys + slot0);
@@ -1306,18 +1358,19 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
   const int64_t nbs = S >> 2;  // buckets per slice
   const uint64_t nb_mask = (uint64_t)(t.cap >> 2) - 1;
   const int max_probes = min(t.probe_limit, kSliceProbes);
-  const int lane = threadIdx.x & 31;
   bool hit_limit = false;
-  for (int64_t k = 0; k < n_stages; ++k) {
-    const uint64_t* st = stage + (size_t)(k & 1) * NS * B;
-    if (k + 1 < n_stages) {
-      slice_stage_copy<NS, B>(si, base, (k + 1) * B, n, stage + (size_t)((k + 1) & 1) * NS * B);
+  __syncthreads();  // the slice is loaded; from here on each warp runs on its own until the store-back
+  for (int j = 0; j < my_blocks; ++j) {
+    const int64_t r0 = ((int64_t)j * kSliceWarps + warp) * WR;
+    const uint64_t* st = ring + (size_t)(j % kSliceRing) * NS * WR;
+    if (j + 1 < my_blocks) {
+      slice_warp_copy<NS, WR>(si, base, r0 + (int64_t)kSliceWarps * WR, n, ring + (size_t)((j + 1) % kSliceRing) * NS * WR, lane);
       asm volatile("cp.async.wait_group 1;" ::: "memory");
     } else {
       asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
-    __syncthreads();  // this stage's rows (and, the first time, the slice) are visible to every thread
-    const int m = (int)min((int64_t)B, n - k * B);
+    __syncwarp();  // this block's rows, copied by every lane, are visible to the whole warp
+    const int m = (int)min((int64_t)WR, n - r0);
     // phase 1: the first bucket of every row, then the slots
     uint64_t key[RPT];
     int64_t lb[RPT];
@@ -1325,8 +1378,8 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
     uint32_t probe = 0;  // rows with a key to probe (the EMPTY pattern is deferred)
 #pragma unroll
     for (int r = 0; r < RPT; ++r) {
-      const int i = threadIdx.x + r * kSliceBlock;
-      key[r] = i < m ? stage_row_key<B>(p, st, i) : kEmptyKey;
+      const int i = lane + 32 * r;
+      key[r] = i < m ? stage_row_key<WR>(p, st, i) : kEmptyKey;
       lb[r] = 0;
       kb[r].x = kb[r].y = kb[r].z = kb[r].w = 0;
       if (i < m && key[r] != kEmptyKey) {
@@ -1335,23 +1388,24 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
         kb[r] = lds_bucket(skeys + 4 * lb[r]);
       }
     }
-    int64_t slot[RPT];
+    int slot[RPT];
 #pragma unroll
     for (int r = 0; r < RPT; ++r) {
       slot[r] = -1;
       if (!((probe >> r) & 1)) continue;
       const int mt = bucket_match(kb[r], key[r]);
       if (mt >= 0) {
-        slot[r] = 4 * lb[r] + mt;
+        slot[r] = (int)(4 * lb[r] + mt);
       } else {
-        slot[r] = slice_probe(skeys, key[r], lb[r], kb[r], nbs, max_probes, &s_fill, fill_limit);
-        if (slot[r] == -2) { hit_limit = true; slot[r] = -1; }
+        const int64_t s = slice_probe(skeys, key[r], lb[r], kb[r], nbs, max_probes, &s_fill, fill_limit);
+        if (s == -2) hit_limit = true;
+        slot[r] = s < 0 ? -1 : (int)s;
       }
     }
     // the deferred rows (live, no slot), reserved once per warp and row position
 #pragma unroll
     for (int r = 0; r < RPT; ++r) {
-      const int i = threadIdx.x + r * kSliceBlock;
+      const int i = lane + 32 * r;
       const bool defer = i < m && slot[r] < 0;
       const unsigned dm = __ballot_sync(0xffffffffu, defer);
       if (dm) {
@@ -1360,29 +1414,19 @@ __device__ __forceinline__ void slice_agg_body(const AggKernelParams& p, const S
         d = __shfl_sync(0xffffffffu, d, 0) + __popc(dm & ((1u << lane) - 1));
         if (defer) {
 #pragma unroll
-          for (int s = 0; s < NS; ++s) si.deferred[s][d] = st[(size_t)s * B + i];
+          for (int s = 0; s < NS; ++s) si.deferred[s][d] = st[(size_t)s * WR + i];
         }
       }
     }
-    // phase 2: the updates, each one for all of the thread's rows
+    // phase 2: the updates of every row and state word
     uint32_t on = 0;
 #pragma unroll
     for (int r = 0; r < RPT; ++r)
       if (slot[r] >= 0) on |= 1u << r;
+    constexpr int G = kSliceUpdPairs / RPT;
     PLN_UNROLL
-    for (int u = 0; u < PLN(n_updates); ++u) {
-      const UpdateDev ud = PLN(upd[u]);
-      uint64_t v[RPT];
-      uint64_t* w[RPT];
-#pragma unroll
-      for (int r = 0; r < RPT; ++r) {
-        const bool has = (on >> r) & 1;
-        v[r] = has ? st[(size_t)ud.slot * B + threadIdx.x + r * kSliceBlock] : 0;
-        w[r] = sst + (has ? slot[r] : 0) * nw + ud.word;
-      }
-      slice_update<RPT>(ud.op, w, v, on);
-    }
-    __syncthreads();  // every thread is done with this buffer before the copy issued in the next stage overwrites it
+    for (int u0 = 0; u0 < PLN(n_updates); u0 += G) slice_update_words<RPT, G, WR>(p, u0, st, lane, sst, nw, slot, on);
+    __syncwarp();  // every lane is done with this buffer before the warp's next copy overwrites it
   }
   const int any_hit = __syncthreads_or(hit_limit);
 #pragma unroll 2

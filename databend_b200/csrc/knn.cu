@@ -143,30 +143,83 @@ __global__ void rerank_kernel(int kind, const float* queries, const float* corpu
   }
 }
 // Certificate of exactness.  Every corpus row that is NOT among a query's candidates has an
-// approximate similarity <= bound[q]; the bf16 rounding of both operands changes a dot product
-// by at most 2^-7 * |q||c| (two relative errors of 2^-8, Cauchy-Schwarz), so such a row's exact
-// similarity is <= bound + E.  If the k-th returned row is better than that, the candidate set
-// provably contained the exact top k; otherwise the query is re-done on the exact path.
+// approximate similarity <= bound[q] (it was filtered against a boundary that only rises, or cut
+// below the k'-th best).  If E bounds (exact similarity - approximate similarity) plus the f32
+// error of the distance the ranking uses, and the k-th returned row beats bound + E, the candidate
+// set provably held the exact top k; otherwise the query is re-done on the exact path.
+//
+// Error budget (u = 2^-8 for bf16 round-to-nearest-even, f32 unit 2^-24, n = dim):
+//  * bf16 operands: RNE moves a value by at most u/(1+u) of itself, either way, so a product
+//    moves by at most (1 + u/(1+u))^2 - 1 = 0.0077972 of |q_i c_i| (a product of two values
+//    rounded up; two values rounded down give 1 - (1+u)^-2 = 0.0077670), and by Cauchy-Schwarz
+//    the dot product by 0.0077972 |q||c|;
+//  * the f32 accumulation inside wgmma (bf16 products are exact in f32): the tensor core's adder
+//    is NOT assumed to round to nearest.  The budget assumes each product enters the accumulator
+//    truncated by less than one f32 ulp of the running magnitude and each accumulate truncates
+//    once more, i.e. at most 2 n 2^-23 sum|q^_i c^_i| <= 2 n 2^-23 * 1.008 |q||c|;
+//  * normalisation (cosine, prep_rows_kernel): rsqrtf (2 ulp), the lane-strided f32 sum of
+//    squares (n/32 + 6 roundings) and the scaling multiply, both operands:
+//    2^-21 + (n/32 + 8) 2^-24;
+//  * the f32 distance the ranking uses (exact_cosine_g8: chains of n/8 + 13 roundings for ab, aa,
+//    bb, then sqrt, mul, div, sub): 2 (n/8 + 13) 2^-24 + 4 2^-24; exact_l2: n + 3 roundings of
+//    non-negative terms, i.e. a relative error of the squared distance below (n + 16) 2^-23;
+//  * 32 2^-24 (cosine) / n 2^-120 (L2, absolute) for the f32 compare and subnormal flushes.
+// The constants are computed for the corpus's dim on the host (certificate_constants).  The budget
+// holds for rows whose squared norms are in range (prep_rows_kernel): a query out of range, or a
+// corpus with a row out of range that is not NaN for every query, is answered exactly.
+struct KnnCertificate {
+  float cos_margin;  // cosine: certified iff 1 - d_k >= bound + cos_margin
+  float l2_cross;    // L2: e = l2_cross |q| cmax + l2_norms (|q|^2 + cmax^2) + l2_floor (1 + |q|)
+  float l2_norms;
+  float l2_floor;
+  float l2_rel;      // L2: certified iff d_k^2 (1 + l2_rel) < -bound - e
+  int corpus_unsafe;
+};
 __global__ void certify_kernel(int kind, int nq, int k, int kk, const int64_t* seg, const float* bound, const float* q_scale,
-                               const unsigned int* max_norm_bits, const float* out_dist, uint8_t* flags) {
+                               const unsigned int* max_norm_bits, const float* out_dist, KnnCertificate cert, uint8_t* flags) {
   for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += gridDim.x * blockDim.x) {
     const int64_t m = seg[q + 1] - seg[q];
+    const float qs = q_scale[q];  // cosine: 1/|q|, L2: |q|^2
+    const bool q_in_range = kind == DBX_DIST_COSINE ? (qs >= 8.8817842e-16f && qs <= 1.1258999e15f)  // 1/|q| in [2^-50, 2^50]
+                                                    : qs <= kCertNormHi;
     bool ok;
     if (m < kk) ok = false;
     else if (kk == 0) ok = true;
-    else if (bound[q] == -INFINITY) ok = true;  // every row with a finite similarity is a candidate
+    else if (cert.corpus_unsafe || !q_in_range) ok = false;
+    else if (bound[q] == -INFINITY) ok = true;  // every row with a non-NaN similarity is a candidate
     else {
       const float dk = out_dist[(int64_t)q * k + kk - 1];
       if (kind == DBX_DIST_COSINE) {
-        ok = (1.0f - dk) >= bound[q] + 0.0079f;
+        ok = (1.0f - dk) >= bound[q] + cert.cos_margin;
       } else {
-        const float qq = q_scale[q], cmax = __uint_as_float(*max_norm_bits);
-        const float e = 0.015640f * sqrtf(qq) * cmax + 2e-5f * (qq + cmax * cmax);
-        ok = dk * dk * 1.00001f <= -bound[q] - e;
+        const float nq_ = sqrtf(qs), cmax = __uint_as_float(*max_norm_bits);
+        const float e = cert.l2_cross * nq_ * cmax + cert.l2_norms * (qs + cmax * cmax) + cert.l2_floor * (1.0f + nq_);
+        ok = dk * dk * (1.0f + cert.l2_rel) < -bound[q] - e;
       }
     }
     flags[q] = ok ? 0 : 1;
   }
+}
+KnnCertificate certificate_constants(int kind, int dim, int corpus_unsafe) {
+  const double n = dim, f32 = std::ldexp(1.0, -24), u = std::ldexp(1.0, -8);
+  const double bf16 = (1.0 + u / (1.0 + u)) * (1.0 + u / (1.0 + u)) - 1.0;  // 0.0077972
+  const double acc = 2.0 * n * std::ldexp(1.0, -23) * 1.008;
+  KnnCertificate c;
+  memset(&c, 0, sizeof(c));
+  c.corpus_unsafe = corpus_unsafe;
+  if (kind == DBX_DIST_COSINE) {
+    const double norm = std::ldexp(1.0, -21) + (n / 32 + 8) * f32;
+    const double exact = (2.0 * (n / 8 + 13) + 4) * f32;
+    c.cos_margin = (float)(bf16 + acc + norm + exact + 32 * f32);
+  } else {
+    // cmax and |q| come from the same f32 sums of squares: (n/32 + 8) 2^-24 relative covers them
+    const double norm_rel = (n / 32 + 8) * f32;
+    c.l2_cross = (float)((2.0 * (bf16 + acc) + std::ldexp(1.0, -21)) * (1.0 + 2.0 * norm_rel));
+    c.l2_norms = (float)(norm_rel + std::ldexp(1.0, -23));
+    c.l2_floor = (float)(n * std::ldexp(1.0, -120));
+    c.l2_rel = (float)((n + 16) * std::ldexp(1.0, -23));
+  }
+  return c;
 }
 // exact path: keys of one query's distances to every corpus row
 // After a similarity pass without a host check: a pass that appended more than the list holds is
@@ -423,6 +476,7 @@ struct dbx_knn {
   DevBuf q_f32, q_bf16, q_scale, bound, seg, seg_off, cand_key[2], cand_row[2], counters, perm[2], key_tmp, sort_alt, dist, qcount;
   DevBuf out_idx_dev, out_dist_dev, max_norm, flags, ex_dist, ex_key[2], ex_row[2], ex_tmp;
   PinnedBuf host, host_flags;
+  int corpus_unsafe = 0;  // rows outside the certificate's norm range (prep_rows_kernel)
   int64_t stat_certified = 0, stat_exact = 0, stat_candidates = 0, stat_passes = 0, stat_cluster = 0, stat_grid = 0, stat_us_passes = 0, stat_us_rerank = 0;
   int64_t cand_cap = 0;
   int64_t last_gemm_launches = 0;
@@ -557,17 +611,20 @@ int32_t dbx_knn_create(int32_t kind, int32_t device, const dbx_column* corpus, d
   DBX_CUDA_TRY(err, cudaMemsetAsync(h->corpus_bf16.p, 0, (size_t)n_alloc * h->dim_pad * 2, h->stream));
   DBX_CUDA_TRY(err, h->c_scale.ensure((size_t)n_alloc * 4));
   DBX_CUDA_TRY(err, cudaMemsetAsync(h->c_scale.p, 0, (size_t)n_alloc * 4, h->stream));
-  DBX_CUDA_TRY(err, h->max_norm.ensure(4));
-  DBX_CUDA_TRY(err, cudaMemsetAsync(h->max_norm.p, 0, 4, h->stream));
+  DBX_CUDA_TRY(err, h->max_norm.ensure(8));  // [0] largest row norm (bits), [1] rows outside the certificate's range
+  DBX_CUDA_TRY(err, cudaMemsetAsync(h->max_norm.p, 0, 8, h->stream));
   if (h->n) {
     prep_rows_kernel<<<grid_1d(h->n * 32), 256, 0, h->stream>>>(h->corpus, h->n, h->dim, h->dim_pad, (__nv_bfloat16*)h->corpus_bf16.p,
-                                                              (float*)h->c_scale.p, kind, (unsigned int*)h->max_norm.p);
+                                                              (float*)h->c_scale.p, kind, (unsigned int*)h->max_norm.p,
+                                                              (unsigned int*)h->max_norm.p + 1);
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
   }
   DBX_CUDA_TRY(err, h->counters.ensure(64));
   DBX_CUDA_TRY(err, h->host.ensure(64));
+  DBX_CUDA_TRY(err, cudaMemcpyAsync(h->host.p, h->max_norm.p, 8, cudaMemcpyDeviceToHost, h->stream));
   DBX_CUDA_TRY(err, cudaStreamSynchronize(h->stream));
+  h->corpus_unsafe = ((const unsigned int*)h->host.p)[1] != 0;
   *out = h.release();
   return DBX_OK;
 }
@@ -627,7 +684,7 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   DBX_CUDA_TRY(err, cudaMemcpyAsync(h->q_f32.p, queries->data, (size_t)nq * dim * 4,
                                     queries->mem == DBX_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
   prep_rows_kernel<<<grid_1d((int64_t)nq_pad * 32), 256, 0, st>>>((const float*)h->q_f32.p, nq_pad, dim, dim_pad, (__nv_bfloat16*)h->q_bf16.p,
-                                                                (float*)h->q_scale.p, h->kind, nullptr);
+                                                                (float*)h->q_scale.p, h->kind, nullptr, nullptr);
   count_launch();
 
   // ---- candidate storage
@@ -861,7 +918,8 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   DBX_CUDA_TRY(err, h->flags.ensure((size_t)nq));
   DBX_CUDA_TRY(err, h->host_flags.ensure((size_t)nq));
   certify_kernel<<<grid_1d(nq), 256, 0, st>>>(h->kind, nq, k, kk, (const int64_t*)h->seg.p, (const float*)h->bound.p, (const float*)h->q_scale.p,
-                                             (const unsigned int*)h->max_norm.p, (const float*)h->out_dist_dev.p, (uint8_t*)h->flags.p);
+                                             (const unsigned int*)h->max_norm.p, (const float*)h->out_dist_dev.p,
+                                             certificate_constants(h->kind, dim, h->corpus_unsafe), (uint8_t*)h->flags.p);
   count_launch();
   DBX_CUDA_TRY(err, cudaGetLastError());
   DBX_CUDA_TRY(err, cudaMemcpyAsync(h->host_flags.p, h->flags.p, (size_t)nq, cudaMemcpyDeviceToHost, st));

@@ -163,17 +163,35 @@ __global__ void distance_rows_kernel(int kind, const float* lhs, int lhs_const, 
 // A zero vector becomes a NaN operand row: its similarities are NaN and never pass the filter.
 // max_norm_bits (optional): bit pattern of the largest row norm (non-negative floats order like
 // their bit patterns), the corpus-side constant of the L2 certificate.
+//
+// The certificate's error budget holds only for rows whose squared norm |x|^2 lies in
+// [2^-100, 2^100] (cosine) or is at most 2^100 (L2): outside it the f32 sums underflow or
+// overflow, and the bf16 operand can become inf / NaN or lose all precision while the exact
+// distance stays finite.  Rows whose exact distance is NaN for every query are harmless (they rank
+// last and the candidate pass never needs them): for cosine a row with a NaN / inf component or no
+// non-zero component, for L2 a row with a NaN component.  unsafe_rows (optional) counts the other
+// rows outside the range; a corpus with any of them gets no certificate.
+constexpr float kCertNormLo = 7.8886091e-31f;  // 2^-100
+constexpr float kCertNormHi = 1.2676506e30f;   // 2^100
 __global__ void prep_rows_kernel(const float* src, int64_t rows, int dim, int dim_pad, __nv_bfloat16* dst, float* scale,
-                                 int kind, unsigned int* max_norm_bits) {
+                                 int kind, unsigned int* max_norm_bits, unsigned int* unsafe_rows) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   float wmax = 0.0f;
+  unsigned int n_unsafe = 0;
   for (int64_t r = warp; r < rows; r += n_warps) {
     const float* a = src + r * dim;
     __nv_bfloat16* d = dst + r * dim_pad;
     float s = 0.0f;
-    for (int i = lane; i < dim; i += 32) { const float x = a[i]; s += x * x; }
+    bool has_nan = false, has_inf = false, has_nonzero = false;
+    for (int i = lane; i < dim; i += 32) {
+      const float x = a[i];
+      s += x * x;
+      has_nan |= x != x;
+      has_inf |= fabsf(x) == INFINITY;
+      has_nonzero |= x != 0.0f;
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     const float mul = kind == DBX_DIST_COSINE ? rsqrtf(s) : 1.0f;
@@ -181,10 +199,19 @@ __global__ void prep_rows_kernel(const float* src, int64_t rows, int dim, int di
       const float x0 = i < dim ? a[i] * mul : 0.0f, x1 = i + 1 < dim ? a[i + 1] * mul : 0.0f;
       *reinterpret_cast<__nv_bfloat162*>(d + i) = __floats2bfloat162_rn(x0, x1);
     }
+    if (unsafe_rows) {
+      has_nan = __any_sync(0xffffffffu, has_nan);
+      has_inf = __any_sync(0xffffffffu, has_inf);
+      has_nonzero = __any_sync(0xffffffffu, has_nonzero);
+      const bool harmless = kind == DBX_DIST_COSINE ? (has_nan || has_inf || !has_nonzero) : has_nan;
+      const bool in_range = kind == DBX_DIST_COSINE ? (s >= kCertNormLo && s <= kCertNormHi) : s <= kCertNormHi;
+      n_unsafe += (!harmless && !in_range) ? 1u : 0u;
+    }
     if (lane == 0) scale[r] = kind == DBX_DIST_COSINE ? mul : s;
     if (s == s) wmax = fmaxf(wmax, sqrtf(s));
   }
   if (max_norm_bits && lane == 0 && wmax > 0.0f) atomicMax(max_norm_bits, __float_as_uint(wmax));
+  if (unsafe_rows && lane == 0 && n_unsafe) atomicAdd(unsafe_rows, n_unsafe);
 }
 
 // ---------------------------------------------------------------- wgmma GEMM with fused filter

@@ -188,7 +188,7 @@ class RfInfo(C.Structure):
 
 EXPR_COLUMN, EXPR_CONST, EXPR_CAST, EXPR_CALL = 0, 1, 2, 3
 (FN_PLUS, FN_MINUS, FN_MULTIPLY, FN_DIVIDE, FN_DIV, FN_MODULO, FN_NEGATE, FN_EQ, FN_NOTEQ, FN_LT, FN_LTE, FN_GT, FN_GTE, FN_AND, FN_OR, FN_NOT,
- FN_IS_NULL, FN_IS_NOT_NULL) = range(18)
+ FN_IS_NULL, FN_IS_NOT_NULL, FN_IF, FN_ASSUME_NOT_NULL) = range(20)
 MAX_EXPR_NODES = 32
 MAX_COMPUTED_COLS = 4
 

@@ -400,6 +400,7 @@ int32_t allocate_slots(AggPlan* pl, ErrorSink* err) {
     CompDev& cd = pl->comp[k];
     memset(&cd, 0, sizeof(cd));
     cd.first = pl->n_cnodes; cd.n_nodes = pl->comp_n_nodes[c]; cd.slot = phys[v];
+    cd.branches = expr_has_branches(pl->comp_nodes[c], pl->comp_n_nodes[c]) ? 1 : 0;
     for (int i = 0; i < pl->comp_n_nodes[c]; ++i) {
       NodeDev nd = pl->comp_nodes[c][i];
       if (nd.kind == DBX_EXPR_COLUMN) nd.col = phys[pl->slot_of(nd.col, err)];

@@ -66,36 +66,42 @@ inline int type_modulo(int a, int b) {
 inline int type_negate(int a) { return is_float_t(a) ? a : make_type(next_bits(bits_of_t(a)), true, false); }
 
 // The interpreter: an 8-deep value stack held in registers (push / pop shift the registers, so no
-// dynamically indexed local array), top of stack in s0.
+// dynamically indexed local array), top of stack in s0.  Every slot carries its own error code in its
+// flag (eval_kernels.cuh: flag_if), so a call on a branch the row does not take does not raise.
 __global__ void __launch_bounds__(256) eval_kernel(const __grid_constant__ EvalParams p) {
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows; r += (int64_t)gridDim.x * blockDim.x) {
     uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0;
-    bool n0 = false, n1 = false, n2 = false, n3 = false, n4 = false, n5 = false, n6 = false, n7 = false;
-    int err = 0;
+    uint32_t f0 = 0, f1 = 0, f2 = 0, f3 = 0, f4 = 0, f5 = 0, f6 = 0, f7 = 0;
     for (int i = 0; i < p.n_nodes; ++i) {
       const NodeDev& nd = p.nodes[i];
       if (nd.kind == DBX_EXPR_COLUMN || nd.kind == DBX_EXPR_CONST) {
         s7 = s6; s6 = s5; s5 = s4; s4 = s3; s3 = s2; s2 = s1; s1 = s0;
-        n7 = n6; n6 = n5; n5 = n4; n4 = n3; n3 = n2; n2 = n1; n1 = n0;
-        if (nd.kind == DBX_EXPR_COLUMN) load_column(p.cols[nd.col], r, nd.out, s0, n0);
-        else { s0 = nd.c_bits; n0 = !nd.c_null; }
-      } else if (nd.kind == DBX_EXPR_CAST) {
-        apply_cast(nd, s0, n0, err);
-      } else if (nd.func == DBX_FN_NOT || nd.func == DBX_FN_NEGATE || nd.func == DBX_FN_IS_NULL || nd.func == DBX_FN_IS_NOT_NULL) {
-        apply_unary(nd, s0, n0, err);
+        f7 = f6; f6 = f5; f5 = f4; f4 = f3; f3 = f2; f2 = f1; f1 = f0;
+        bool ok = !nd.c_null;
+        if (nd.kind == DBX_EXPR_COLUMN) load_column(p.cols[nd.col], r, nd.out, s0, ok);
+        else s0 = ok ? nd.c_bits : 0;
+        f0 = ok;
+      } else if (nd.kind == DBX_EXPR_CAST || is_unary_call(nd.func)) {
+        flag_cast_unary(nd, s0, f0);
+      } else if (nd.func == DBX_FN_IF) {
+        flag_if(s2, f2, s1, f1, s0, f0);  // if(s2, s1, s0) -> s2, then pop two
+        s0 = s2; s1 = s3; s2 = s4; s3 = s5; s4 = s6; s5 = s7;
+        f0 = f2; f1 = f3; f2 = f4; f3 = f5; f4 = f6; f5 = f7;
       } else {
-        apply_binary(nd, s1, n1, s0, n0, err);  // s1 op s0 -> s1, then pop
+        flag_binary(nd, s1, f1, s0, f0);
         s0 = s1; s1 = s2; s2 = s3; s3 = s4; s4 = s5; s5 = s6; s6 = s7;
-        n0 = n1; n1 = n2; n2 = n3; n3 = n4; n4 = n5; n5 = n6; n6 = n7;
+        f0 = f1; f1 = f2; f2 = f3; f3 = f4; f4 = f5; f5 = f6; f6 = f7;
       }
     }
-    store_result(p, r, s0, n0, err);
+    store_result(p, r, s0, f0 & 1, (int)(f0 >> 1));
   }
 }
 
 // Source of the straight-line kernel for a type-checked program: every node is a constexpr
-// NodeDev, every stack slot a named variable.
+// NodeDev, every stack slot a named variable.  Programs with IF / ASSUME_NOT_NULL carry one flag
+// (validity | error code << 1) per slot; the others keep one error register for the whole row.
 std::string specialised_source(const EvalParams& p) {
+  const bool cond = expr_has_branches(p.nodes, p.n_nodes);
   std::ostringstream o;
   o << "#define DBX_JIT 1\n#include \"eval_kernels.cuh\"\nnamespace dbx {\n__device__ constexpr NodeDev jnodes[" << p.n_nodes << "] = {\n";
   for (int i = 0; i < p.n_nodes; ++i) {
@@ -107,20 +113,36 @@ std::string specialised_source(const EvalParams& p) {
   }
   o << "};\n}\nextern \"C\" __global__ void __launch_bounds__(256) dbx_jit_eval(const __grid_constant__ dbx::EvalParams p) {\n"
     << "  using namespace dbx;\n"
-    << "  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows; r += (int64_t)gridDim.x * blockDim.x) {\n"
-    << "    int err = 0;\n";
-  for (int d = 0; d < kEvalStack; ++d) o << "    uint64_t v" << d << " = 0; bool k" << d << " = false;\n";
+    << "  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows; r += (int64_t)gridDim.x * blockDim.x) {\n";
+  if (cond) {
+    for (int d = 0; d < kEvalStack; ++d) o << "    uint64_t v" << d << " = 0; uint32_t f" << d << " = 0; bool k" << d << " = false;\n";
+  } else {
+    o << "    int err = 0;\n";
+    for (int d = 0; d < kEvalStack; ++d) o << "    uint64_t v" << d << " = 0; bool k" << d << " = false;\n";
+  }
   int sp = 0;
   for (int i = 0; i < p.n_nodes; ++i) {
     const NodeDev& n = p.nodes[i];
-    if (n.kind == DBX_EXPR_COLUMN) { o << "    load_column(p.cols[" << n.col << "], r, " << n.out << ", v" << sp << ", k" << sp << ");\n"; ++sp; }
-    else if (n.kind == DBX_EXPR_CONST) { o << "    v" << sp << " = jnodes[" << i << "].c_bits; k" << sp << " = !jnodes[" << i << "].c_null;\n"; ++sp; }
-    else if (n.kind == DBX_EXPR_CAST) o << "    apply_cast(jnodes[" << i << "], v" << sp - 1 << ", k" << sp - 1 << ", err);\n";
-    else if (n.func == DBX_FN_NOT || n.func == DBX_FN_NEGATE || n.func == DBX_FN_IS_NULL || n.func == DBX_FN_IS_NOT_NULL)
-      o << "    apply_unary(jnodes[" << i << "], v" << sp - 1 << ", k" << sp - 1 << ", err);\n";
-    else { o << "    apply_binary(jnodes[" << i << "], v" << sp - 2 << ", k" << sp - 2 << ", v" << sp - 1 << ", k" << sp - 1 << ", err);\n"; --sp; }
+    const std::string nd = "jnodes[" + std::to_string(i) + "]";
+    if (n.kind == DBX_EXPR_COLUMN) {
+      o << "    load_column(p.cols[" << n.col << "], r, " << n.out << ", v" << sp << ", k" << sp << ");\n";
+      if (cond) o << "    f" << sp << " = k" << sp << ";\n";
+      ++sp;
+    } else if (n.kind == DBX_EXPR_CONST) {
+      if (cond) o << "    f" << sp << " = !" << nd << ".c_null; v" << sp << " = f" << sp << " ? " << nd << ".c_bits : 0;\n";
+      else o << "    v" << sp << " = " << nd << ".c_bits; k" << sp << " = !" << nd << ".c_null;\n";
+      ++sp;
+    } else if (cond) {
+      if (n.kind == DBX_EXPR_CAST || is_unary_call(n.func)) o << "    flag_cast_unary(" << nd << ", v" << sp - 1 << ", f" << sp - 1 << ");\n";
+      else if (n.func == DBX_FN_IF) { o << "    flag_if(v" << sp - 3 << ", f" << sp - 3 << ", v" << sp - 2 << ", f" << sp - 2 << ", v" << sp - 1 << ", f" << sp - 1 << ");\n"; sp -= 2; }
+      else { o << "    flag_binary(" << nd << ", v" << sp - 2 << ", f" << sp - 2 << ", v" << sp - 1 << ", f" << sp - 1 << ");\n"; --sp; }
+    }
+    else if (n.kind == DBX_EXPR_CAST) o << "    apply_cast(" << nd << ", v" << sp - 1 << ", k" << sp - 1 << ", err);\n";
+    else if (is_unary_call(n.func)) o << "    apply_unary(" << nd << ", v" << sp - 1 << ", k" << sp - 1 << ", err);\n";
+    else { o << "    apply_binary(" << nd << ", v" << sp - 2 << ", k" << sp - 2 << ", v" << sp - 1 << ", k" << sp - 1 << ", err);\n"; --sp; }
   }
-  o << "    store_result(p, r, v0, k0, err);\n  }\n}\n";
+  if (cond) o << "    store_result(p, r, v0, f0 & 1, (int)(f0 >> 1));\n  }\n}\n";
+  else o << "    store_result(p, r, v0, k0, err);\n  }\n}\n";
   return o.str();
 }
 
@@ -160,15 +182,26 @@ int32_t infer_expr_types(const dbx_expr& expr, int n_cols, const int* col_dtype,
       tstack[sp - 1] = to; nstack[sp - 1] = nstack[sp - 1] || in.try_cast;
     } else if (in.kind == DBX_EXPR_CALL) {
       const int f = in.func;
-      const bool unary = f == DBX_FN_NOT || f == DBX_FN_NEGATE || f == DBX_FN_IS_NULL || f == DBX_FN_IS_NOT_NULL;
-      if (sp < (unary ? 1 : 2)) { err.set("eval: malformed postfix program"); return DBX_ERR_INVALID; }
+      const bool unary = is_unary_call(f);
+      if (sp < (unary ? 1 : f == DBX_FN_IF ? 3 : 2)) { err.set("eval: malformed postfix program"); return DBX_ERR_INVALID; }
       if (unary) {
         const int ta = tstack[sp - 1];
         nd.a_type = ta;
         if (f == DBX_FN_NOT) { if (ta != DBX_BOOL) { err.set("eval: not() needs a Boolean argument"); return DBX_ERR_INVALID; } nd.out = DBX_BOOL; }
         else if (f == DBX_FN_NEGATE) { if (!numeric(ta)) { err.set("eval: minus() needs a numeric argument"); return DBX_ERR_INVALID; } nd.out = type_negate(ta); }
+        else if (f == DBX_FN_ASSUME_NOT_NULL) { nd.out = ta; nstack[sp - 1] = false; }
         else { nd.out = DBX_BOOL; nstack[sp - 1] = false; }
         tstack[sp - 1] = nd.out;
+        continue;
+      }
+      if (f == DBX_FN_IF) {  // if(cond: Boolean NULL, then: T0, else: T0) -> T0 (control.rs:36-108)
+        const int tc = tstack[sp - 3], tt = tstack[sp - 2], te = tstack[sp - 1];
+        if (tc != DBX_BOOL) { err.set("eval: if() needs a Boolean condition"); return DBX_ERR_INVALID; }
+        if (tt != te) { err.set("eval: if() branches must have one type (the type checker casts every branch to their common super type: add DBX_EXPR_CAST nodes; a NULL literal carries the branch type)"); return DBX_ERR_INVALID; }
+        nd.a_type = tc; nd.b_type = tt; nd.out = tt;
+        const bool nullable = nstack[sp - 2] || nstack[sp - 1];
+        sp -= 2;
+        tstack[sp - 1] = tt; nstack[sp - 1] = nullable;
         continue;
       }
       const int ta = tstack[sp - 2], tb = tstack[sp - 1];
@@ -228,6 +261,12 @@ bool expr_can_raise(const NodeDev* nodes, int n_nodes) {
       if (!const_divisor || (!d.c_null && zero)) return true;
     }
   }
+  return false;
+}
+
+bool expr_has_branches(const NodeDev* nodes, int n_nodes) {
+  for (int i = 0; i < n_nodes; ++i)
+    if (nodes[i].kind == DBX_EXPR_CALL && (nodes[i].func == DBX_FN_IF || nodes[i].func == DBX_FN_ASSUME_NOT_NULL)) return true;
   return false;
 }
 
@@ -360,8 +399,9 @@ extern "C" int32_t dbx_eval_scalar(int32_t device, const dbx_expr* expr, const d
   return rc;
 }
 
-// Generates and compiles (no GPU needed) the straight-line kernel of a canned program that touches
-// every node kind: cast(c0 % 7 as Int64) > -cast(c1 as Int64) and not(is_null(c1)).
+// Generates and compiles (no GPU needed) the straight-line kernels of two canned programs that touch
+// every node kind: b = cast(c0 % 7 as Int64) > -cast(c1 as Int64) and not(is_null(c1)), and the
+// conditional if(b, assume_not_null(c1), 0.0).
 extern "C" int32_t dbx_eval_jit_selftest(char* msg, int32_t msg_cap) {
   EvalParams p;
   memset(&p, 0, sizeof(p));
@@ -386,7 +426,14 @@ extern "C" int32_t dbx_eval_jit_selftest(char* msg, int32_t msg_cap) {
   p.out_dtype = DBX_BOOL;
   std::string why;
   cudaKernel_t k = nullptr;
-  const bool ok = jit_get_kernel(specialised_source(p), "dbx_jit_eval", &k, &why, /*compile_only=*/true);
+  bool ok = jit_get_kernel(specialised_source(p), "dbx_jit_eval", &k, &why, /*compile_only=*/true);
+  node(DBX_EXPR_COLUMN, 0, 1, DBX_F64, 0, 0, 0, 0);
+  node(DBX_EXPR_CALL, DBX_FN_ASSUME_NOT_NULL, 0, DBX_F64, DBX_F64, 0, 0, 0);
+  node(DBX_EXPR_CONST, 0, 0, DBX_F64, 0, 0, 0, 0);
+  node(DBX_EXPR_CALL, DBX_FN_IF, 0, DBX_F64, DBX_BOOL, DBX_F64, 0, 0);
+  p.n_nodes = i;
+  p.out_dtype = DBX_F64;
+  ok = ok && jit_get_kernel(specialised_source(p), "dbx_jit_eval", &k, &why, /*compile_only=*/true);
   if (msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", ok ? "ok" : why.c_str());
   return ok ? DBX_OK : DBX_ERR_UNSUPPORTED;
 }

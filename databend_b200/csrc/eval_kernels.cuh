@@ -261,6 +261,37 @@ __device__ __forceinline__ void store_result(const EvalParams& p, int64_t r, uin
   if (p.out_valid) p.out_valid[r] = valid ? 1 : 0;
 }
 
+// ---- conditional programs (IF / ASSUME_NOT_NULL, evaluator.rs:1702-1790 eval_if).  A call on a branch the
+// row does not take must not raise on it, so each stack slot carries the code of the first failing call of
+// its own subtree next to its validity: flag = valid | code << 1.  A call's code is `a ?: b ?: own`, the
+// first in program order, which is what the single `err` of the evaluators above computes for programs
+// without these nodes (they keep that form: one error register instead of one per slot).
+__host__ __device__ inline bool is_unary_call(int f) {
+  return f == DBX_FN_NOT || f == DBX_FN_NEGATE || f == DBX_FN_IS_NULL || f == DBX_FN_IS_NOT_NULL || f == DBX_FN_ASSUME_NOT_NULL;
+}
+__device__ __forceinline__ void flag_cast_unary(const NodeDev& nd, uint64_t& a, uint32_t& af) {
+  bool an = af & 1;
+  int err = (int)(af >> 1);
+  if (nd.kind == DBX_EXPR_CAST) apply_cast(nd, a, an, err);
+  else if (nd.func == DBX_FN_ASSUME_NOT_NULL) { a = an ? a : 0; an = true; }  // other.rs:217-229: the type's default under a NULL
+  else apply_unary(nd, a, an, err);
+  af = (uint32_t)an | ((uint32_t)err << 1);
+}
+__device__ __forceinline__ void flag_binary(const NodeDev& nd, uint64_t& a, uint32_t& af, const uint64_t b, const uint32_t bf) {
+  bool an = af & 1;
+  int err = (int)((af >> 1) ? (af >> 1) : (bf >> 1));
+  apply_binary(nd, a, an, b, (bf & 1) != 0, err);
+  af = (uint32_t)an | ((uint32_t)err << 1);
+}
+// if(c, t, e) -> c: both branches were evaluated; the row takes `t` when c is true (a NULL condition is
+// false) and keeps the taken branch's value, validity and code behind the condition's own code
+__device__ __forceinline__ void flag_if(uint64_t& c, uint32_t& cf, const uint64_t t, const uint32_t tf, const uint64_t e, const uint32_t ef) {
+  const bool take = (cf & 1) && c != 0;
+  const uint32_t sf = take ? tf : ef;
+  c = take ? t : e;
+  cf = (cf >> 1) ? ((cf & ~1u) | (sf & 1)) : sf;
+}
+
 #ifndef DBX_JIT
 // The reference's type inference over a postfix program (arithmetics_type.rs): fills nodes[i] (types of
 // every node; COLUMN nodes keep the column index in `col`) and the result type and nullability.  Columns
@@ -272,6 +303,8 @@ int32_t infer_expr_types(const dbx_expr& expr, int n_cols, const int* col_dtype,
 // `/`, `div` or `%` whose divisor is not a non-zero constant, a non-try cast that can overflow, or a
 // negation of an Int64 / UInt64
 bool expr_can_raise(const NodeDev* nodes, int n_nodes);
+// true when the program has an IF or ASSUME_NOT_NULL node: it is evaluated with per-slot error codes
+bool expr_has_branches(const NodeDev* nodes, int n_nodes);
 #endif
 
 }  // namespace dbx

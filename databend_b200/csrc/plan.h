@@ -161,7 +161,7 @@ struct KeyPartDev {
 struct CompDev {
   int32_t first, n_nodes;
   int32_t slot;
-  int32_t pad;
+  int32_t branches;  // 1: the program has IF / ASSUME_NOT_NULL (evaluated by comp_row_cond)
 };
 
 struct AggKernelParams {

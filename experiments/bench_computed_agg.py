@@ -70,11 +70,22 @@ def materialise(blk, exprs):
     return DataBlock(cols, blk.num_rows), dts, t
 
 
-def shape(name, n, blk, types, params_f, params_m, filt, exprs, in_bytes, reps):
+def same_results(a, b):
+    return all(np.allclose(np.sort(a.columns[i].values()), np.sort(b.columns[i].values()), rtol=1e-9, equal_nan=True)
+               for i in range(a.num_columns()))
+
+
+def shape(name, n, blk, types, params_f, params_m, filt, exprs, in_bytes, reps, params_a=None):
+    """params_a: an optional third variant, a fused form of the same query written without IF."""
     for _ in range(2):
         run(params_f, filt, blk, types)
     runs = [run(params_f, filt, blk, types) for _ in range(reps)]
     tf, kf, out_f = min(r[0] for r in runs), min(r[1] for r in runs), runs[-1][2]
+    variants = []
+    if params_a is not None:
+        run(params_a, filt, blk, types)
+        runs_a = [run(params_a, filt, blk, types) for _ in range(reps)]
+        variants.append(("fused-arith", min(r[0] for r in runs_a), min(r[1] for r in runs_a), in_bytes, same_results(out_f, runs_a[-1][2])))
     tm_best, km_best, out_m = None, None, None
     for _ in range(reps + 1):
         mblk, dts, t_eval = materialise(blk, exprs)
@@ -82,9 +93,8 @@ def shape(name, n, blk, types, params_f, params_m, filt, exprs, in_bytes, reps):
         tm_best = t_eval + t_agg if tm_best is None else min(tm_best, t_eval + t_agg)
         km_best = k_agg if km_best is None else min(km_best, k_agg)
         del mblk
-    same = all(np.allclose(np.sort(out_f.columns[i].values()), np.sort(out_m.columns[i].values()), rtol=1e-9, equal_nan=True)
-               for i in range(out_f.num_columns()))
-    for how, t, k, bpr in (("fused", tf, kf, in_bytes), ("materialised", tm_best, km_best, in_bytes + 16 * len(exprs))):
+    same = same_results(out_f, out_m)
+    for how, t, k, bpr, same in [("fused", tf, kf, in_bytes, same), ("materialised", tm_best, km_best, in_bytes + 16 * len(exprs), same)] + variants:
         print(f"{name:10s} {how:13s} rows {n:.3g}  query {t * 1e3:9.2f} ms  {n / t / 1e9:7.2f} G rows/s  {bpr:3d} B/row  "
               f"query share of HBM bound {n * bpr / t / HBM_BPS:5.2f}  aggregate kernel {k:8.2f} ms (events)  results equal: {same}")
 
@@ -128,6 +138,30 @@ def main():
     filt = E.eq(E.col(1) % E.lit(3), E.lit(0))
     shape("1e6-group", n, blk, types, AggregatorParams([0], [("sum", e1), ("avg", e2)]), AggregatorParams([0], [("sum", 3), ("avg", 4)]),
           filt, [e1, e2], 24, a.reps)
+    del blk, cols
+    # Q12-shaped (ship modes and priorities as integer codes): SELECT mode, sum(if(prio = 0 or prio = 1, 1, 0)),
+    # sum(if(prio > 1, 1, 0)) WHERE (mode = 0 OR mode = 1) AND receipt < 1000 GROUP BY mode
+    cols = [dev_col(0, 31, 7, n, abi.I64), dev_col(0, 32, 5, n, abi.I64), dev_col(0, 33, 2600, n, abi.I64)]
+    blk = DataBlock(cols, n)
+    types = [abi.I64] * 3
+    zero, one64 = S.lit(0, abi.I64), S.lit(1, abi.I64)
+    high = S.call("or", S.call("eq", S.col(1), zero), S.call("eq", S.col(1), one64))
+    low = S.call("gt", S.col(1), one64)
+    h, lo = S.if_(high, one64, zero), S.if_(low, one64, zero)
+    filt = E.and_(E.or_(E.eq(E.col(0), E.lit(0)), E.eq(E.col(0), E.lit(1))), E.lt(E.col(2), E.lit(1000)))
+    shape("Q12", n, blk, types, AggregatorParams([0], [("sum", h), ("sum", lo)]), AggregatorParams([0], [("sum", 3), ("sum", 4)]), filt,
+          [h, lo], 24, a.reps, AggregatorParams([0], [("sum", S.cast(high, abi.I64)), ("sum", S.cast(low, abi.I64))]))
+    del blk, cols
+    # Q14-shaped, no GROUP BY: sum(if(ptype < 25, price * (1 - disc), 0.0)), sum(price * (1 - disc)) over a ship-date range
+    cols = [dev_col(2, 41, 17, n, abi.F64), dev_col(3, 42, 0, n, abi.F64), dev_col(0, 43, 150, n, abi.I64), dev_col(0, 44, 2600, n, abi.I64)]
+    blk = DataBlock(cols, n)
+    types = [abi.F64, abi.F64, abi.I64, abi.I64]
+    rev = S.col(0) * (one - S.col(1))
+    promo_c = S.call("lt", S.col(2), S.lit(25, abi.I64))
+    promo = S.if_(promo_c, rev, S.lit(0.0, abi.F64))
+    filt = E.and_(E.ge(E.col(3), E.lit(1000)), E.lt(E.col(3), E.lit(1030)))
+    shape("Q14", n, blk, types, AggregatorParams([], [("sum", promo), ("sum", rev)]), AggregatorParams([], [("sum", 4), ("sum", 5)]), filt,
+          [promo, rev], 32, a.reps, AggregatorParams([], [("sum", rev * S.cast(promo_c, abi.F64)), ("sum", rev)]))
 
 
 if __name__ == "__main__":

@@ -543,11 +543,26 @@ typedef enum dbx_expr_kind { DBX_EXPR_COLUMN = 0, DBX_EXPR_CONST = 1, DBX_EXPR_C
 typedef enum dbx_func {
   DBX_FN_PLUS = 0, DBX_FN_MINUS = 1, DBX_FN_MULTIPLY = 2, DBX_FN_DIVIDE = 3, DBX_FN_DIV = 4, DBX_FN_MODULO = 5, DBX_FN_NEGATE = 6,
   DBX_FN_EQ = 7, DBX_FN_NOTEQ = 8, DBX_FN_LT = 9, DBX_FN_LTE = 10, DBX_FN_GT = 11, DBX_FN_GTE = 12,
-  DBX_FN_AND = 13, DBX_FN_OR = 14, DBX_FN_NOT = 15, DBX_FN_IS_NULL = 16, DBX_FN_IS_NOT_NULL = 17
+  DBX_FN_AND = 13, DBX_FN_OR = 14, DBX_FN_NOT = 15, DBX_FN_IS_NULL = 16, DBX_FN_IS_NOT_NULL = 17,
+  DBX_FN_IF = 18, DBX_FN_ASSUME_NOT_NULL = 19
 } dbx_func;
+/* Conditionals.  Every conditional SQL form binds to the reference's `if(c1, r1, ..., cm, rm, else)`
+ * (CASE, coalesce, nullif, iff, ifnull / nvl, nvl2, IS [NOT] DISTINCT FROM: sql/.../type_check/
+ * scalar_rewrite.rs, special_function.rs, rewrite_function.rs).  It is sent as its arguments in postfix
+ * order followed by m consecutive DBX_FN_IF nodes, i.e. if(c1, r1, if(c2, r2, ... else)) — equal in value,
+ * type, nullability and errors.
+ *   DBX_FN_IF (3 arguments: cond, then, else; control.rs:36-108): cond must be DBX_BOOL, nullable or not;
+ *     then and else must have one dtype (the caller adds the cast nodes, as for comparisons; a NULL literal
+ *     carries the branch dtype).  The result has that dtype and is nullable when either branch is.  A NULL
+ *     condition counts as false.  Lazy like eval_if (evaluator.rs:1702-1790): a call raises only on rows
+ *     that reach it — the condition on every row that reaches the IF, a branch only on rows that take it.
+ *   DBX_FN_ASSUME_NOT_NULL (1 argument; other.rs:217-229): the argument without its validity; on a NULL
+ *     row the value is unspecified (the device gives the type's default, 0).
+ * Anything else is DBX_ERR_INVALID with a message that says so.  The 8-deep value stack and the 32-node
+ * limit hold for conditionals too: a 3-arm CASE fits, a deeper one is DBX_ERR_UNSUPPORTED. */
 typedef struct dbx_expr_node {
   int32_t kind;     /* dbx_expr_kind */
-  int32_t func;     /* dbx_func (DBX_EXPR_CALL); arguments are the 1 or 2 values below it on the stack */
+  int32_t func;     /* dbx_func (DBX_EXPR_CALL); arguments are the 1, 2 or 3 values below it on the stack */
   int32_t col;      /* DBX_EXPR_COLUMN: column index in the block */
   int32_t cast_to;  /* DBX_EXPR_CAST: dbx_dtype */
   int32_t try_cast; /* DBX_EXPR_CAST: 1 = try_to_<type> (failure gives NULL instead of an error) */

@@ -34,10 +34,19 @@ namespace dbx {
 namespace {
 
 // ================================================================ key images
+// Key classes: VC_INT / VC_UINT / VC_FLT (Float64 bits) and KC_F32, a Float32 key carried in its own
+// 32 bits.  A float -> double -> float round trip quiets a signalling NaN on sm_90 (0x7F800001 comes
+// back as 0x7FC00001), and the result must return every row's key bit for bit.
+constexpr int KC_F32 = 3;
+inline int key_class(int dtype) {
+  if (dtype == DBX_F32) return KC_F32;
+  return dtype == DBX_U64 ? VC_UINT : (dtype_class(dtype) == VC_FLT ? VC_FLT : VC_INT);
+}
+
 __device__ __forceinline__ uint64_t key_to_ord(uint64_t bits, int cls, bool asc) {
   uint64_t o;
-  if (cls == VC_FLT) {
-    double d = __longlong_as_double((long long)bits);
+  if (cls == VC_FLT || cls == KC_F32) {
+    double d = cls == KC_F32 ? (double)__uint_as_float((uint32_t)bits) : __longlong_as_double((long long)bits);
     if (d == 0.0) d = 0.0;  // -0 == +0
     o = f64_to_ordered(d);
   } else if (cls == VC_INT) {
@@ -48,13 +57,13 @@ __device__ __forceinline__ uint64_t key_to_ord(uint64_t bits, int cls, bool asc)
   return asc ? o : ~o;
 }
 
+// integers sign- or zero-extended to 64 bits; Float32 keeps its own 32 bits (see KC_F32)
 __device__ __forceinline__ uint64_t load_widened(const DevCol& c, int64_t row, uint64_t pol) {
   const char* base = (const char*)c.data;
   switch (c.dtype) {
     case DBX_I64: case DBX_U64: case DBX_F64: return ld_stream_u64(base + row * 8, pol);
     case DBX_I32: return (uint64_t)(int64_t)(int32_t)ld_stream_u32(base + row * 4, pol);
-    case DBX_U32: return ld_stream_u32(base + row * 4, pol);
-    case DBX_F32: return (uint64_t)__double_as_longlong((double)__uint_as_float(ld_stream_u32(base + row * 4, pol)));
+    case DBX_U32: case DBX_F32: return ld_stream_u32(base + row * 4, pol);
     case DBX_I16: return (uint64_t)(int64_t)(int16_t)ld_stream_u16(base + row * 2, pol);
     case DBX_U16: return ld_stream_u16(base + row * 2, pol);
     case DBX_I8: return (uint64_t)(int64_t)(int8_t)ld_stream_u8(base + row, pol);
@@ -66,8 +75,7 @@ __device__ __forceinline__ void store_narrow_key(void* out, int64_t i, int dtype
   switch (dtype) {
     case DBX_I8: case DBX_U8: ((uint8_t*)out)[i] = (uint8_t)b; break;
     case DBX_I16: case DBX_U16: ((uint16_t*)out)[i] = (uint16_t)b; break;
-    case DBX_I32: case DBX_U32: ((uint32_t*)out)[i] = (uint32_t)b; break;
-    case DBX_F32: ((float*)out)[i] = (float)__longlong_as_double((long long)b); break;
+    case DBX_I32: case DBX_U32: case DBX_F32: ((uint32_t*)out)[i] = (uint32_t)b; break;
     default: ((uint64_t*)out)[i] = b; break;
   }
 }
@@ -453,6 +461,9 @@ __global__ void __launch_bounds__(256) sort_ingest_kernel(const __grid_constant_
     if (ok && cls == VC_FLT) {
       const double d = __longlong_as_double((long long)v);
       lossy |= (d != d && v != 0x7FF8000000000000ULL) || (d == 0.0 && (v >> 63));
+    } else if (ok && cls == KC_F32) {
+      const float f = __uint_as_float((uint32_t)v);
+      lossy |= (f != f && v != 0x7FC00000u) || (f == 0.0f && (v >> 31));
     }
   }
   if (inexact && __any_sync(0xffffffffu, lossy) && (threadIdx.x & 31) == 0) *inexact = 1;
@@ -491,7 +502,12 @@ __global__ void sort_emit_kernel(const __grid_constant__ SortEmitArgs a) {
       if (a.bits) b = a.bits[row];
       else {
         const uint64_t o = a.asc ? a.ord[i] : ~a.ord[i];
-        b = a.cls == VC_FLT ? (uint64_t)__double_as_longlong(ordered_to_f64(o)) : (a.cls == VC_INT ? o ^ 0x8000000000000000ULL : o);
+        if (a.cls == KC_F32) {  // the image of a NaN decodes to the canonical 0x7FC00000 (others are gathered)
+          const double d = ordered_to_f64(o);
+          b = d != d ? 0x7FC00000u : __float_as_uint((float)d);
+        } else {
+          b = a.cls == VC_FLT ? (uint64_t)__double_as_longlong(ordered_to_f64(o)) : (a.cls == VC_INT ? o ^ 0x8000000000000000ULL : o);
+        }
       }
     }
     store_narrow_key(a.out_key, i, a.dtype, b);
@@ -547,8 +563,8 @@ __device__ __forceinline__ uint64_t key_field(uint64_t v, int dtype, int width, 
     double d = __longlong_as_double((long long)v);
     if (d == 0.0) d = 0.0;  // -0 == +0
     o = f64_to_ordered(d);
-  } else if (dtype == DBX_F32) {  // the same order as the widened value
-    float f = (float)__longlong_as_double((long long)v);
+  } else if (dtype == DBX_F32) {
+    float f = __uint_as_float((uint32_t)v);
     uint32_t u;
     if (f != f) u = 0xFFFFFFFFu;
     else {
@@ -616,7 +632,7 @@ __device__ __forceinline__ bool multi_row(const MultiKeys& mk, int64_t r, bool o
 struct MultiList {
   uint64_t* img;    // [W][cap]: image word w of entry i at img[w * cap + i]
   uint64_t* rowid;  // global row ordinal
-  uint64_t* bits;   // the first key's original value bits (widened), 0 for NULL
+  uint64_t* bits;   // the first key's original value bits (as load_widened returns them), 0 for NULL
   unsigned long long* state;  // MST_* words
   int64_t cap;
 };
@@ -1002,8 +1018,8 @@ class TopkOp : public Op {
     key_dtype = types[p->key_col] & 0xFF;
     key_nullable = (types[p->key_col] & DBX_NULLABLE) != 0;
     if (dtype_size(key_dtype) == 0) { err.set("top-k: key must be a numeric column"); return DBX_ERR_UNSUPPORTED; }
-    cls = key_dtype == DBX_U64 ? VC_UINT : (dtype_class(key_dtype) == VC_FLT ? VC_FLT : VC_INT);
-    full_sort = p->limit == 0 || p->limit > (1 << 22);  // no LIMIT (or one too large for the candidate list): sort everything
+    cls = key_class(key_dtype);
+    full_sort = p->limit == 0 || p->limit > (1 << 22);  // no LIMIT (or one too large for the candidate list): sort everything, then cut
     n_extra = p->n_extra_keys;
     if (n_extra < 0 || n_extra > DBX_MAX_SORT_KEYS - 1) { err.set("sort: at most 4 sort keys"); return DBX_ERR_INVALID; }
     for (int j = 0; j < n_extra; ++j) {
@@ -1012,7 +1028,7 @@ class TopkOp : public Op {
       x_dtype[j] = types[c] & 0xFF;
       x_nullable[j] = (types[c] & DBX_NULLABLE) != 0;
       if (dtype_size(x_dtype[j]) == 0) { err.set("sort: keys must be numeric columns"); return DBX_ERR_UNSUPPORTED; }
-      x_cls[j] = x_dtype[j] == DBX_U64 ? VC_UINT : (dtype_class(x_dtype[j]) == VC_FLT ? VC_FLT : VC_INT);
+      x_cls[j] = key_class(x_dtype[j]);
     }
     // several keys with a LIMIT: streaming top-k over the composite order image
     multi = n_extra > 0 && !full_sort;
@@ -1431,7 +1447,9 @@ class TopkOp : public Op {
     }
     if (!sorted_ord) { sorted_ord = (const uint64_t*)s_ord[buf].p; sorted_rid = (const uint32_t*)s_rid[buf].p; }
     const int64_t n_in = n;
-    const int64_t n_out = (n_extra > 0 && prm.limit > 0) ? std::min<int64_t>(n_in, prm.limit) : n_in;
+    const int64_t n_out = prm.limit > 0 ? std::min<int64_t>(n_in, prm.limit) : n_in;  // LIMIT > 4 Mi: cut the sorted rows
+    // the first key's NULL rows are one run at the start (NULLS FIRST) or the end of the sorted rows
+    const int64_t out_nulls = prm.nulls_first ? std::min(n_nulls, n_out) : std::max<int64_t>(0, n_out - (n_in - n_nulls));
     void *okey = nullptr, *orow = nullptr, *ovb = nullptr, *obits = nullptr;
     const int esz = dtype_size(key_dtype);
     DBX_TRY(dev_alloc(ob.get(), (size_t)n_out * esz, &okey));
@@ -1456,7 +1474,7 @@ class TopkOp : public Op {
     dbx_column kcol;
     memset(&kcol, 0, sizeof(kcol));
     kcol.dtype = key_dtype; kcol.mem = DBX_MEM_DEVICE; kcol.len = n_out; kcol.data = okey;
-    if (key_nullable) { kcol.validity = (const uint8_t*)obits; kcol.null_count = n_out == n_in ? n_nulls : -1; }
+    if (key_nullable) { kcol.validity = (const uint8_t*)obits; kcol.null_count = out_nulls; }
     dbx_column rcol;
     memset(&rcol, 0, sizeof(rcol));
     rcol.dtype = DBX_I64; rcol.mem = DBX_MEM_DEVICE; rcol.len = n_out; rcol.data = orow;

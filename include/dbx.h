@@ -186,7 +186,9 @@ typedef struct dbx_agg_params {
 /* SortColumnDescription{offset, asc, nulls_first} + LimitType::{LimitRows(k), None}
  * (kernels/sort.rs:41-63).  Order: OrderedFloat (NaN greatest, -0 == +0); ties keep row order.
  * limit = 0 (LimitType::None) sorts the whole input (device radix sort, up to 2^30 - 1 rows);
- * 1 <= limit <= 4 Mi runs the streaming top-k.  Result block: [key, row_id Int64]. */
+ * 1 <= limit <= 4 Mi runs the streaming top-k; limit > 4 Mi sorts the whole input and cuts the
+ * result to `limit` rows.  Result block: [key, row_id Int64], min(n, limit) rows for limit > 0;
+ * the key keeps each row's value bit for bit (NaN sign and payload, -0.0). */
 #define DBX_MAX_SORT_KEYS 4
 typedef struct dbx_topk_params {
   int32_t key_col;
@@ -201,7 +203,7 @@ typedef struct dbx_topk_params {
    * bit if nullable, then the order-preserving value at its natural width; at most 5 x 64 bits),
    * with no row limit; with limit = 0 or limit > 4 Mi the whole input is sorted on the device (one
    * stable radix sort per key, least significant first, up to 2^30 - 1 rows) and `limit` > 0 cuts
-   * the sorted result.  Result block: [key (first key), row_id Int64] as for one key. */
+   * the sorted result, as for one key.  Result block: [key (first key), row_id Int64] as for one key. */
   int32_t n_extra_keys; /* 0 .. DBX_MAX_SORT_KEYS - 1 */
   int32_t extra_key_cols[DBX_MAX_SORT_KEYS - 1];
   int32_t extra_asc[DBX_MAX_SORT_KEYS - 1];

@@ -221,5 +221,5 @@ EXPORTS = [
     "dbx_eval_scalar", "dbx_op_kernel_variant", "dbx_agg_jit_selftest", "dbx_eval_jit_selftest",
     "dbx_agg_partial_serialize", "dbx_agg_final_merge_serialized",
     "dbx_join_runtime_filter", "dbx_runtime_filter_info", "dbx_runtime_filter_export", "dbx_runtime_filter_apply",
-    "dbx_runtime_filter_destroy", "dbx_op_create_computed", "dbx_agg_expr_jit_selftest",
+    "dbx_runtime_filter_destroy", "dbx_op_create_computed", "dbx_agg_expr_jit_selftest", "dbx_op_create_join",
 ]

@@ -195,36 +195,7 @@ __device__ __forceinline__ uint64_t comp_row(const CompDev& cd, const NodeDev* c
   ok = n0;
   return n0 ? s0 : 0;
 }
-// The same for a program with IF / ASSUME_NOT_NULL (CompDev::branches): one flag per slot, validity | error
-// code << 1 (eval_kernels.cuh: flag_if), so only the branch a row takes can raise on it.
-template <typename V>
-__device__ __forceinline__ uint64_t comp_row_cond(const CompDev& cd, const NodeDev* cnodes, const V& v, uint32_t valid, bool& ok, int& err) {
-  uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0;
-  uint32_t f0 = 0, f1 = 0, f2 = 0, f3 = 0, f4 = 0, f5 = 0, f6 = 0, f7 = 0;
-  PLN_UNROLL
-  for (int i = cd.first; i < cd.first + cd.n_nodes; ++i) {
-    const NodeDev nd = cnodes[i];
-    if (nd.kind == DBX_EXPR_COLUMN || nd.kind == DBX_EXPR_CONST) {
-      s7 = s6; s6 = s5; s5 = s4; s4 = s3; s3 = s2; s2 = s1; s1 = s0;
-      f7 = f6; f6 = f5; f5 = f4; f4 = f3; f3 = f2; f2 = f1; f1 = f0;
-      if (nd.kind == DBX_EXPR_COLUMN) { f0 = (valid >> nd.col) & 1; s0 = f0 ? v[nd.col] : 0; }
-      else { f0 = !nd.c_null; s0 = f0 ? nd.c_bits : 0; }
-    } else if (nd.kind == DBX_EXPR_CAST || is_unary_call(nd.func)) {
-      flag_cast_unary(nd, s0, f0);
-    } else if (nd.func == DBX_FN_IF) {
-      flag_if(s2, f2, s1, f1, s0, f0);  // if(s2, s1, s0) -> s2, then pop two
-      s0 = s2; s1 = s3; s2 = s4; s3 = s5; s4 = s6; s5 = s7;
-      f0 = f2; f1 = f3; f2 = f4; f3 = f5; f4 = f6; f5 = f7;
-    } else {
-      flag_binary(nd, s1, f1, s0, f0);  // s1 op s0 -> s1, then pop
-      s0 = s1; s1 = s2; s2 = s3; s3 = s4; s4 = s5; s5 = s6; s6 = s7;
-      f0 = f1; f1 = f2; f2 = f3; f3 = f4; f4 = f5; f5 = f6; f6 = f7;
-    }
-  }
-  ok = f0 & 1;
-  err = (int)(f0 >> 1);
-  return ok ? s0 : 0;
-}
+// The same for a program with IF / ASSUME_NOT_NULL (CompDev::branches) is comp_row_cond (eval_kernels.cuh).
 #ifndef DBX_JIT
 // The precompiled kernels share ONE out-of-line copy of the interpreter (inlined into every
 // instantiation it would multiply their code and build time); a specialised build inlines comp_row

@@ -292,6 +292,57 @@ __device__ __forceinline__ void flag_if(uint64_t& c, uint32_t& cf, const uint64_
   cf = (cf >> 1) ? ((cf & ~1u) | (sf & 1)) : sf;
 }
 
+// One computed column (dbx_op_create_computed) or residual predicate (dbx_op_create_join): the postfix
+// program cnodes[first, first + n_nodes) evaluated per row with the node functions above; COLUMN nodes
+// name a SLOT (NodeDev::col), the value goes to slot `slot` as the 64-bit image load_slot would give a
+// column of its type.
+struct CompDev {
+  int32_t first, n_nodes;
+  int32_t slot;
+  int32_t branches;  // 1: the program has IF / ASSUME_NOT_NULL (evaluated by comp_row_cond)
+};
+
+// The interpreter's node loop unrolls only in a run-time specialised build (DBX_JIT), where the nodes
+// are compile-time constants; the precompiled kernels keep it a loop.
+#ifdef DBX_JIT
+#define COMP_UNROLL _Pragma("unroll")
+#else
+#define COMP_UNROLL
+#endif
+
+// A postfix program on one row: a value stack held in registers (push / pop shift them), COLUMN nodes
+// read the row's slot values v[] / validity bits, one flag per stack slot, validity | error code << 1
+// (flag_if), so only the branch a row takes can raise on it.  Returns the value (0 when NULL).  The
+// fused aggregate kernels (agg_kernels.cuh) and the join's residual predicate (join.cu) run it.
+template <typename V>
+__device__ __forceinline__ uint64_t comp_row_cond(const CompDev& cd, const NodeDev* cnodes, const V& v, uint32_t valid, bool& ok, int& err) {
+  uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0;
+  uint32_t f0 = 0, f1 = 0, f2 = 0, f3 = 0, f4 = 0, f5 = 0, f6 = 0, f7 = 0;
+  COMP_UNROLL
+  for (int i = cd.first; i < cd.first + cd.n_nodes; ++i) {
+    const NodeDev nd = cnodes[i];
+    if (nd.kind == DBX_EXPR_COLUMN || nd.kind == DBX_EXPR_CONST) {
+      s7 = s6; s6 = s5; s5 = s4; s4 = s3; s3 = s2; s2 = s1; s1 = s0;
+      f7 = f6; f6 = f5; f5 = f4; f4 = f3; f3 = f2; f2 = f1; f1 = f0;
+      if (nd.kind == DBX_EXPR_COLUMN) { f0 = (valid >> nd.col) & 1; s0 = f0 ? v[nd.col] : 0; }
+      else { f0 = !nd.c_null; s0 = f0 ? nd.c_bits : 0; }
+    } else if (nd.kind == DBX_EXPR_CAST || is_unary_call(nd.func)) {
+      flag_cast_unary(nd, s0, f0);
+    } else if (nd.func == DBX_FN_IF) {
+      flag_if(s2, f2, s1, f1, s0, f0);  // if(s2, s1, s0) -> s2, then pop two
+      s0 = s2; s1 = s3; s2 = s4; s3 = s5; s4 = s6; s5 = s7;
+      f0 = f2; f1 = f3; f2 = f4; f3 = f5; f4 = f6; f5 = f7;
+    } else {
+      flag_binary(nd, s1, f1, s0, f0);  // s1 op s0 -> s1, then pop
+      s0 = s1; s1 = s2; s2 = s3; s3 = s4; s4 = s5; s5 = s6; s6 = s7;
+      f0 = f1; f1 = f2; f2 = f3; f3 = f4; f4 = f5; f5 = f6; f6 = f7;
+    }
+  }
+  ok = f0 & 1;
+  err = (int)(f0 >> 1);
+  return ok ? s0 : 0;
+}
+
 #ifndef DBX_JIT
 // The reference's type inference over a postfix program (arithmetics_type.rs): fills nodes[i] (types of
 // every node; COLUMN nodes keep the column index in `col`) and the result type and nullability.  Columns

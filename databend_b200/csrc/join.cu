@@ -108,6 +108,19 @@ struct JoinColDev {
                                 // 4 + s: the packed key's bit field at shift s (composite keys)
 };
 
+// One value slot of the residual predicate (RESID kernels): a probe column, read once per probe row,
+// or a build column, read per candidate pair from the source JoinColDev::from names for it.
+constexpr int kResidSlots = 8;  // comp_row_cond's value slots
+struct ResidSlotDev {
+  DevCol probe;                // side 0: the probe block's column
+  const void* src;             // side 1, from = 0: the build column, gathered by build row
+  const uint8_t* valid_bytes;  // side 1, from = 0: one byte per build row, or null (all valid)
+  int32_t side;                // 0 probe, 1 build
+  int32_t from;                // build side: as JoinColDev::from
+  int32_t dtype;
+  int32_t size;
+};
+
 struct JoinProbeParams {
   DevCol key;
   JoinTableDev table;
@@ -122,6 +135,11 @@ struct JoinProbeParams {
   JoinKeyPack pack;            // composite keys (PACKED kernels): the probe key columns
   RfPartDev rf;                // RF kernels: the runtime filter's min-max and bloom (runtime_filter.cuh)
   unsigned long long* rf_rejected;  // RF kernels: rows the filter turned away
+  // RESID kernels (kept behind every field above, so the other kernels see the same layout): the
+  // residual predicate's program, its COLUMN nodes naming slots of resid_slots
+  int32_t resid_n_nodes, resid_n_slots;
+  ResidSlotDev resid_slots[kResidSlots];
+  NodeDev resid_nodes[kMaxExprNodes];
 };
 
 __device__ __forceinline__ uint64_t load_key(const DevCol& c, int64_t row) {
@@ -249,6 +267,74 @@ __device__ __forceinline__ void emit_match(const JoinProbeParams& p, int64_t r, 
   }
 }
 
+// ---- residual predicate (HashJoinDesc::other_predicate, hash_join/desc.rs:156-190): the ON clause's
+// non-equi conditions, evaluated on every candidate pair (equal keys) inside the probe.  A pair whose
+// predicate is NULL or false is no match, for every kind.  The values of one pair sit in up to eight
+// slots: the probe row's are loaded once before its walk, the build row's per candidate from the entry
+// (key, p0, p1, packed key field) or by a gather by build row.
+struct ResidRow { uint64_t v[kResidSlots]; };
+
+// value image (load_image's) of a build value held as its raw bytes, zero-extended: integers sign- or
+// zero-extended to 64 bits, F32 as the f64 bits of its value
+__device__ __forceinline__ uint64_t raw_image(uint64_t raw, int dtype) {
+  if (dtype == DBX_F32) return (uint64_t)__double_as_longlong((double)__uint_as_float((uint32_t)raw));
+  return wrap_int(raw, dtype);
+}
+
+__device__ __forceinline__ void resid_load_probe(const JoinProbeParams& p, int64_t r, ResidRow& row, uint32_t& valid) {
+  valid = 0;
+#pragma unroll
+  for (int s = 0; s < kResidSlots; ++s) {
+    row.v[s] = 0;
+    if (s >= p.resid_n_slots || p.resid_slots[s].side != 0) continue;
+    bool ok;
+    load_column(p.resid_slots[s].probe, r, p.resid_slots[s].dtype, row.v[s], ok);
+    valid |= (ok ? 1u : 0u) << s;
+  }
+}
+
+// The RESID kernels share ONE out-of-line copy of the interpreter, for the reason agg_kernels.cuh's
+// comp_row_interp gives: inlined, it would multiply their code and build time.  NULL counts as false
+// (the reference's is_true wrapper); the predicate cannot raise (dbx_op_create_join refuses such).
+static __device__ __noinline__ bool resid_true(const JoinProbeParams& p, const ResidRow row, uint32_t valid) {
+  bool ok = false;
+  int err = 0;
+  const CompDev cd{0, p.resid_n_nodes, 0, 1};
+  const uint64_t v = comp_row_cond(cd, p.resid_nodes, row.v, valid, ok, err);
+  return ok && v != 0;
+}
+
+// Is the candidate pair (probe row `row`, build entry e) a matching pair?
+template <int KW>
+__device__ __forceinline__ bool resid_match(const JoinProbeParams& p, const JEntry<KW>& e, ResidRow row, uint32_t valid) {
+#pragma unroll
+  for (int s = 0; s < kResidSlots; ++s) {
+    if (s >= p.resid_n_slots || p.resid_slots[s].side == 0) continue;
+    const ResidSlotDev& rs = p.resid_slots[s];
+    uint64_t raw;
+    bool ok = true;
+    if (rs.from == 0) {
+      const int64_t b = (int64_t)(e.row1 & kRowMask) - 1;
+      raw = load_raw(rs.src, rs.size, b);
+      ok = !rs.valid_bytes || rs.valid_bytes[b];
+    } else if (rs.from == 1) {
+      raw = e.key;
+    } else if (rs.from == 2) {
+      raw = e.p0;
+      ok = (e.row1 >> 62) & 1;
+    } else if (rs.from == 3) {
+      raw = entry_p1(e);
+      ok = (e.row1 >> 63) & 1;
+    } else {
+      const int sh = rs.from - 4;
+      raw = (sh < 64 ? e.key : key_hi(e)) >> (sh & 63);
+    }
+    row.v[s] = ok ? raw_image(raw, rs.dtype) : 0;
+    valid |= (ok ? 1u : 0u) << s;
+  }
+  return resid_true(p, row, valid);
+}
+
 // Does any key occur twice on the build side?  One thread per slot walks the rest of the slot's
 // probe sequence (short at load factor <= 0.5).  A build side without duplicates (the usual
 // primary-key dimension table) lets the probe stop at its first match instead of walking on to the
@@ -289,7 +375,13 @@ __global__ void join_dup_check_kernel(const __grid_constant__ JoinTableDev t, un
 // RF (single key): the join's runtime filter tests min-max and bloom before the table walk; a
 // rejected row cannot match and takes the no-match path, which is right for every kind.  The
 // RF = false instantiations carry none of it.
-template <int KW, bool PACKED, bool UNIQUE, bool MARK, bool RF = false>
+// RESID: the residual predicate decides, on every key match (candidate pair), whether the pair is a
+// matching pair; only matching pairs are counted, marked, kept as `first` and emitted, so every kind's
+// rule ("matched", "no match") reads as "has a matching pair".  The probe row's slots are loaded once
+// before the walk; the re-walk evaluates the predicate again and skips the first matching pair.  LEFT
+// SEMI / ANTI without MARK stop at the first matching pair.  The RESID = false instantiations carry none
+// of it.
+template <int KW, bool PACKED, bool UNIQUE, bool MARK, bool RF = false, bool RESID = false>
 __global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 0) join_probe2_kernel(const __grid_constant__ JoinProbeParams p) {
   __shared__ unsigned int s_warp[kJoinBlock / 32];
   __shared__ unsigned long long s_base;
@@ -299,6 +391,8 @@ __global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 
   const int64_t n_iter = (p.n_rows + step - 1) / step;
   const JEntry<KW>* const entries = (const JEntry<KW>*)p.table.entries;
   unsigned int rf_rej = 0;
+  // LEFT SEMI / ANTI only ask whether a matching pair exists (with MARK every match is marked)
+  const bool stop_at_first = UNIQUE || (RESID && !MARK && (p.kind == DBX_JOIN_LEFT_SEMI || p.kind == DBX_JOIN_LEFT_ANTI));
   for (int64_t it = 0; it < n_iter; ++it) {
     int64_t r[2];
     r[0] = it * step + (int64_t)blockIdx.x * blockDim.x * 2 + threadIdx.x;
@@ -308,6 +402,8 @@ __global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 
     int64_t b0[2] = {0, 0}, sl[2] = {0, 0};
     unsigned int n_match[2] = {0, 0};
     JEntry<KW> first[2];
+    ResidRow prow[2];      // RESID: the probe row's slots
+    uint32_t pvalid[2] = {0, 0};
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       clear_entry(first[j]);
@@ -322,6 +418,7 @@ __global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 
         if (!PACKED) k[j] = load_key(p.key, r[j]);
         b0[j] = join_home<KW>(p.table, k[j], kh[j]);
         sl[j] = b0[j];
+        if (RESID) resid_load_probe(p, r[j], prow[j], pvalid[j]);
       }
     }
     while (go[0] || go[1]) {  // an empty entry ends a probe sequence
@@ -334,13 +431,16 @@ __global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 
         if (!go[j]) continue;
         if (e[j].row1 == 0) { go[j] = false; continue; }
         if (key_eq(e[j], k[j], kh[j])) {
-          if (MARK) {  // read first: a dimension row hit by many facts is written once, not per match
-            uint8_t* m = p.matched + (int64_t)(e[j].row1 & kRowMask) - 1;
-            if (*m == 0) *m = 1;
+          if (!RESID || resid_match<KW>(p, e[j], prow[j], pvalid[j])) {
+            if (MARK) {  // read first: a dimension row hit by many facts is written once, not per match
+              uint8_t* m = p.matched + (int64_t)(e[j].row1 & kRowMask) - 1;
+              if (*m == 0) *m = 1;
+            }
+            if (n_match[j] == 0) first[j] = e[j];
+            ++n_match[j];
+            if (stop_at_first) { go[j] = false; continue; }
           }
-          if (n_match[j] == 0) first[j] = e[j];
-          ++n_match[j];
-          if (UNIQUE) { go[j] = false; continue; }
+          if (RESID && UNIQUE) { go[j] = false; continue; }  // the row's only candidate
         }
         sl[j] = (sl[j] + 1) & mask;
       }
@@ -393,7 +493,8 @@ __global__ void __launch_bounds__(kJoinBlock, (PACKED || (RF && !UNIQUE)) ? 3 : 
           for (;;) {
             const JEntry<KW> e = load_entry(entries + b);
             if (e.row1 == 0) break;
-            if (key_eq(e, k[j], kh[j]) && seen++ > 0) emit_match<PACKED>(p, r[j], e, pos++);
+            if (key_eq(e, k[j], kh[j]) && (!RESID || resid_match<KW>(p, e, prow[j], pvalid[j])) && seen++ > 0)
+              emit_match<PACKED>(p, r[j], e, pos++);
             b = (b + 1) & mask;
           }
         }
@@ -718,25 +819,97 @@ class JoinOp : public Op {
     return DBX_OK;
   }
 
-  template <int KW, bool PACKED, bool RF = false>
+  // Residual predicate (dbx_op_create_join): the type-checked program, its COLUMN nodes renumbered to
+  // slots; resid_col[s] = schema column of slot s (build columns, then the probe columns)
+  int resid_n_nodes = 0, resid_n_slots = 0;
+  NodeDev resid_nodes[kMaxExprNodes];
+  int resid_col[kResidSlots];
+
+  int32_t set_residual(const dbx_expr* e) {
+    if (!e || e->n_nodes == 0) return DBX_OK;
+    const int n = n_build_cols + n_probe_cols;
+    int dtypes[2 * kMaxJoinCols];
+    bool nullable[2 * kMaxJoinCols];
+    for (int c = 0; c < n_build_cols; ++c) { dtypes[c] = build_dtype[c]; nullable[c] = build_nullable[c]; }
+    for (int c = 0; c < n_probe_cols; ++c) { dtypes[n_build_cols + c] = probe_dtype[c]; nullable[n_build_cols + c] = probe_nullable[c]; }
+    int dt = 0;
+    bool out_nullable = false;
+    const int32_t st = infer_expr_types(*e, n, dtypes, nullable, resid_nodes, &dt, &out_nullable, err);
+    if (st != DBX_OK) { err.set("join other_predicate: " + err.msg); return st; }
+    if (dt != DBX_BOOL) { err.set("join other_predicate: the predicate must be Boolean (nullable or not)"); return DBX_ERR_INVALID; }
+    if (expr_can_raise(resid_nodes, e->n_nodes)) {
+      err.set("join other_predicate: a predicate that can raise (`/`, `div` or `%` by a non-constant or zero divisor, an overflowing "
+              "cast, a negation of an Int64 / UInt64) is not built: the reference's selector evaluates AND / OR children under an "
+              "adaptive order (expression/src/filter/selector.rs:182-300), so which pairs reach it there is not deterministic");
+      return DBX_ERR_UNSUPPORTED;
+    }
+    int n_slots = 0;
+    for (int i = 0; i < e->n_nodes; ++i) {
+      if (resid_nodes[i].kind != DBX_EXPR_COLUMN) continue;
+      const int c = resid_nodes[i].col;
+      int s = 0;
+      while (s < n_slots && resid_col[s] != c) ++s;
+      if (s == n_slots) {
+        if (n_slots == kResidSlots) {
+          err.set("join other_predicate: the predicate references more than 8 distinct columns (the interpreter has 8 value slots)");
+          return DBX_ERR_UNSUPPORTED;
+        }
+        resid_col[n_slots++] = c;
+      }
+      resid_nodes[i].col = s;
+    }
+    resid_n_nodes = e->n_nodes;
+    resid_n_slots = n_slots;
+    return DBX_OK;
+  }
+  // the device slot table of one probe block (probe columns `cols`)
+  void fill_residual(JoinProbeParams& pp, const DevCol* cols) {
+    pp.resid_n_nodes = resid_n_nodes;
+    pp.resid_n_slots = resid_n_slots;
+    memcpy(pp.resid_nodes, resid_nodes, sizeof(NodeDev) * resid_n_nodes);
+    for (int s = 0; s < resid_n_slots; ++s) {
+      ResidSlotDev& rs = pp.resid_slots[s];
+      const int c = resid_col[s];
+      if (c >= n_build_cols) {
+        rs.side = 0;
+        rs.probe = cols[c - n_build_cols];
+        rs.dtype = probe_dtype[c - n_build_cols];
+        continue;
+      }
+      rs.side = 1;
+      rs.dtype = build_dtype[c];
+      rs.size = build[c].size;
+      if (packed && build_key_shift(c) >= 0) rs.from = 4 + build_key_shift(c);  // the packed key's field
+      else rs.from = c == prm.build_key_col ? 1 : (c == inline_col[0] ? 2 : (c == inline_col[1] ? 3 : 0));
+      rs.src = build[c].data.p;
+      rs.valid_bytes = build[c].nullable ? (const uint8_t*)build[c].valid_bytes.p : nullptr;
+    }
+  }
+
+  template <int KW, bool PACKED, bool RF = false, bool RESID = false>
   void launch_probe2(const JoinProbeParams& pp, int grid) {
     if (pp.matched) {
-      if (build_unique) join_probe2_kernel<KW, PACKED, true, true, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
-      else join_probe2_kernel<KW, PACKED, false, true, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
+      if (build_unique) join_probe2_kernel<KW, PACKED, true, true, RF, RESID><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<KW, PACKED, false, true, RF, RESID><<<grid, kJoinBlock, 0, stream>>>(pp);
     } else {
-      if (build_unique) join_probe2_kernel<KW, PACKED, true, false, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
-      else join_probe2_kernel<KW, PACKED, false, false, RF><<<grid, kJoinBlock, 0, stream>>>(pp);
+      if (build_unique) join_probe2_kernel<KW, PACKED, true, false, RF, RESID><<<grid, kJoinBlock, 0, stream>>>(pp);
+      else join_probe2_kernel<KW, PACKED, false, false, RF, RESID><<<grid, kJoinBlock, 0, stream>>>(pp);
     }
+  }
+  template <bool RESID>
+  void launch_probe_as(const JoinProbeParams& pp, int grid) {
+    if (packed) {
+      if (key_words == 2) launch_probe2<2, true, false, RESID>(pp, grid);
+      else launch_probe2<1, true, false, RESID>(pp, grid);
+      return;
+    }
+    if (rf_probe) { launch_probe2<1, false, true, RESID>(pp, grid); return; }
+    launch_probe2<1, false, false, RESID>(pp, grid);
   }
   void launch_probe(const JoinProbeParams& pp, int64_t rows) {
     const int grid = grid_rows((rows + 1) / 2);
-    if (packed) {
-      if (key_words == 2) launch_probe2<2, true>(pp, grid);
-      else launch_probe2<1, true>(pp, grid);
-      return;
-    }
-    if (rf_probe) { launch_probe2<1, false, true>(pp, grid); return; }
-    launch_probe2<1, false>(pp, grid);
+    if (resid_n_nodes) launch_probe_as<true>(pp, grid);
+    else launch_probe_as<false>(pp, grid);
   }
 
   // Join::probe_block: join one probe block; the joined block is queued for dbx_op_pull
@@ -784,6 +957,7 @@ class JoinOp : public Op {
           pp.pack.parts[i] = probe_part[i];
         }
       }
+      if (resid_n_nodes) fill_residual(pp, cols);
       std::vector<uint8_t*> valid_bytes;
       auto add_out = [&](JoinColDev& jc, int dtype, bool nullable) -> int32_t {
         void* d = nullptr;
@@ -1023,6 +1197,23 @@ Op* make_join_op(const dbx_join_params* p, const int32_t* types, int32_t n, int 
 }  // namespace dbx
 
 using namespace dbx;
+
+extern "C" int32_t dbx_op_create_join(const dbx_join_params* params, const int32_t* input_types, int32_t n_input_cols,
+                                      const dbx_expr* other_predicate, int32_t device, dbx_op** out) {
+  if (!out || !params || !input_types) { g_create_error.set("dbx_op_create_join: null argument"); return DBX_ERR_INVALID; }
+  *out = nullptr;
+  int32_t ndev = 0;
+  DBX_TRY(dbx_device_count(&ndev));
+  if (device < 0 || device >= ndev) { g_create_error.set("dbx_op_create: device index out of range"); return DBX_ERR_INVALID; }
+  int32_t st = DBX_OK;
+  Op* op = make_join_op(params, input_types, n_input_cols, device, &st);
+  if (!op) return st == DBX_OK ? DBX_ERR_INVALID : st;
+  st = static_cast<JoinOp*>(op)->set_residual(other_predicate);
+  if (st != DBX_OK) { g_create_error.set(op->err.msg); delete op; return st; }
+  op->kind = DBX_OP_JOIN;
+  *out = reinterpret_cast<dbx_op*>(op);
+  return DBX_OK;
+}
 
 extern "C" int32_t dbx_join_probe(dbx_op* op, const dbx_block* block) {
   if (!op || !block) return DBX_ERR_INVALID;

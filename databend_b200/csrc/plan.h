@@ -155,15 +155,6 @@ struct KeyPartDev {
   uint64_t mask;       // value field mask (unshifted)
 };
 
-// One computed column (dbx_op_create_computed): the postfix program cnodes[first, first + n_nodes)
-// evaluated per row with eval_kernels.cuh's node functions; COLUMN nodes name a SLOT (NodeDev::col),
-// the value goes to slot `slot` as the 64-bit image load_slot would give a column of its type.
-struct CompDev {
-  int32_t first, n_nodes;
-  int32_t slot;
-  int32_t branches;  // 1: the program has IF / ASSUME_NOT_NULL (evaluated by comp_row_cond)
-};
-
 struct AggKernelParams {
   DevCol cols[kMaxSlots];
   PredNodeDev nodes[DBX_MAX_PRED_NODES];

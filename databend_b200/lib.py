@@ -111,6 +111,7 @@ def load():
         "dbx_runtime_filter_destroy": (i32, [vp]),
         "dbx_op_create_computed": (i32, [i32, vp, P(i32), i32, P(abi.Expr), i32, i32, P(vp)]),
         "dbx_agg_expr_jit_selftest": (i32, [C.c_char_p, i32]),
+        "dbx_op_create_join": (i32, [P(abi.JoinParams), P(i32), i32, P(abi.Expr), i32, P(vp)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)  # AttributeError = the library does not export a declared symbol

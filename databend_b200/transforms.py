@@ -413,7 +413,8 @@ class HashJoin(_Op):
     unspecified (compare as multisets)."""
 
     def __init__(self, build_types: Sequence[int], probe_types: Sequence[int], build_key: Union[int, Sequence[int]],
-                 probe_key: Union[int, Sequence[int]], device: int = 0, kind: int = abi.JOIN_INNER, expected_build_rows: int = 0):
+                 probe_key: Union[int, Sequence[int]], device: int = 0, kind: int = abi.JOIN_INNER, expected_build_rows: int = 0,
+                 other_predicate: Optional[S.SExpr] = None):
         """kind (probe side = left, build side = right):
           JOIN_INNER, JOIN_LEFT (probe rows kept), JOIN_LEFT_SEMI / JOIN_LEFT_ANTI (probe columns only:
           left_join_semi.rs / left_join_anti.rs);
@@ -422,7 +423,11 @@ class HashJoin(_Op):
           (LEFT during the probe, then RIGHT's final stream).
         build_key / probe_key: one column index each, or equally long sequences of up to
         abi.MAX_JOIN_KEYS indices (ON b[0] = p[0] AND b[1] = p[1] ...; a NULL in any key column never
-        matches).  The keys are packed into 64 or 128 bits (join_key_layout)."""
+        matches).  The keys are packed into 64 or 128 bits (join_key_layout).
+        other_predicate: the ON clause's non-equi conditions ANDed together (HashJoinDesc::other_predicate), a
+        Boolean scalar_expr.SExpr whose column i is build column i for i < len(build_types) and probe column
+        i - len(build_types) above.  It is evaluated on every pair of equal keys inside the probe; a pair on
+        which it is NULL or false is no match, for every kind (include/dbx.h: dbx_op_create_join)."""
         bkeys, pkeys = _key_list(build_key), _key_list(probe_key)
         if len(bkeys) != len(pkeys) or not 1 <= len(bkeys) <= abi.MAX_JOIN_KEYS:
             raise DbxError(abi.ERR_INVALID, f"join: build and probe keys must be 1 .. {abi.MAX_JOIN_KEYS} columns each, as many on both sides")
@@ -432,7 +437,16 @@ class HashJoin(_Op):
         p.n_extra_keys = len(bkeys) - 1
         for i in range(1, len(bkeys)):
             p.extra_build_key_cols[i - 1], p.extra_probe_key_cols[i - 1] = bkeys[i], pkeys[i]
-        super().__init__(abi.OP_JOIN, p, list(build_types) + list(probe_types), device)
+        types = list(build_types) + list(probe_types)
+        if other_predicate is None:
+            super().__init__(abi.OP_JOIN, p, types, device)
+            return
+        self._h = C.c_void_p()
+        self.device = device
+        self._params = p
+        self._predicate = S.flatten(other_predicate)
+        ctypes_ = (C.c_int32 * len(types))(*types)
+        check(load().dbx_op_create_join(C.byref(p), ctypes_, len(types), C.byref(self._predicate), device, C.byref(self._h)))
 
     def add_block(self, block: DataBlock):
         self.push(block)

@@ -353,6 +353,37 @@ typedef struct dbx_expr dbx_expr;
 int32_t dbx_op_create_computed(int32_t kind, const void* params, const int32_t* input_types, int32_t n_input_cols,
                                const dbx_expr* computed, int32_t n_computed, int32_t device, dbx_op** out);
 
+/* Join::probe with HashJoinDesc::other_predicate (hash_join/desc.rs:156-190): a join whose ON clause has
+ * non-equi conditions next to its key equalities (band joins, `t1.b > t2.b`, TPC-H Q21's `<>`).
+ * `params`, `input_types` and every other call are as for dbx_op_create(DBX_OP_JOIN, ...);
+ * other_predicate == NULL or n_nodes == 0 is that join.  other_predicate is a dbx_expr (see
+ * dbx_eval_scalar) of the non-equi conditions ANDed together:
+ *   Columns: DBX_EXPR_COLUMN indices address input_types as the join lays it out: build column c is
+ *     c (0 .. n_build_cols - 1), probe column j is n_build_cols + j.
+ *   Nullability comes from the DBX_NULLABLE flags of input_types (the rule of computed columns).
+ *   Type: the predicate must infer to DBX_BOOL, nullable or not; anything else, and a column outside
+ *     the schema, is DBX_ERR_INVALID.  A NULL result counts as false (the reference's is_true wrapper).
+ *   DBX_ERR_UNSUPPORTED, with the reason in dbx_last_error(NULL):
+ *     - a predicate that can raise (`/`, `div` or `%` whose divisor is not a non-zero constant, a non-try
+ *       cast that can overflow, a negation of an Int64 / UInt64), for the reason given for predicate
+ *       computed columns: the reference's selector evaluates AND / OR children under an adaptive order,
+ *       so which pairs reach a raising call there is not deterministic;
+ *     - a predicate that references more than 8 distinct columns (the interpreter's 8 value slots).
+ * A candidate pair is a probe row and a build row with equal keys; a matching pair is a candidate pair
+ * on which the predicate is true.  Each kind then reads "match" as "matching pair":
+ *   INNER       probe blocks emit every matching pair;
+ *   LEFT        every matching pair, and each probe row with no matching pair once, build columns NULL;
+ *   LEFT SEMI   each probe row with at least one matching pair, once;
+ *   LEFT ANTI   each probe row with no matching pair (NULL-key rows included);
+ *   RIGHT       probe blocks: every matching pair; final_probe: the build rows in no matching pair;
+ *   RIGHT SEMI / RIGHT ANTI  final_probe: the build rows in at least one / in no matching pair;
+ *   FULL        probe blocks as LEFT, final_probe as RIGHT.
+ * Output columns, their nullability and the (unspecified) row order are those of the join without a
+ * predicate.  dbx_op_reset keeps the predicate.  Runtime filters (dbx_join_runtime_filter, _apply and
+ * in_probe) work as without it: a probe row the filter rejects has no candidate pair. */
+int32_t dbx_op_create_join(const dbx_join_params* params, const int32_t* input_types, int32_t n_input_cols,
+                           const dbx_expr* other_predicate, int32_t device, dbx_op** out);
+
 /* Join probe side: Join::probe_block(block) -> JoinStream::next()* ; output blocks are
  * pulled with dbx_op_pull until drained. */
 int32_t dbx_join_probe(dbx_op* op, const dbx_block* block);

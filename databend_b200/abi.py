@@ -11,7 +11,7 @@ ABI_VERSION = 1
 OK, ERR_INVALID, ERR_CUDA, ERR_BAD_ARGUMENTS, ERR_UNSUPPORTED, ERR_OOM, ERR_STATE, ERR_NO_DEVICE = range(8)
 
 # dbx_dtype
-BOOL, I8, I16, I32, I64, U8, U16, U32, U64, F32, F64, VEC_F32 = range(12)
+BOOL, I8, I16, I32, I64, U8, U16, U32, U64, F32, F64, VEC_F32, VEC_I8 = range(13)
 MEM_HOST, MEM_DEVICE = 0, 1
 NULLABLE = 0x100
 

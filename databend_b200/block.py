@@ -29,8 +29,9 @@ _DBX2NP = {v: k for k, v in _NP2DBX.items()}
 DTYPE_NAMES = {
     abi.BOOL: "Boolean", abi.I8: "Int8", abi.I16: "Int16", abi.I32: "Int32", abi.I64: "Int64",
     abi.U8: "UInt8", abi.U16: "UInt16", abi.U32: "UInt32", abi.U64: "UInt64",
-    abi.F32: "Float32", abi.F64: "Float64", abi.VEC_F32: "Vector(Float32)",
+    abi.F32: "Float32", abi.F64: "Float64", abi.VEC_F32: "Vector(Float32)", abi.VEC_I8: "Vector(Int8)",
 }
+_VEC_ELEM = {abi.VEC_F32: np.dtype(np.float32), abi.VEC_I8: np.dtype(np.int8)}
 
 
 def np_dtype(dbx_dtype: int) -> np.dtype:
@@ -126,6 +127,16 @@ class Column:
         return Column(abi.VEC_F32, arr.shape[0], data=arr, vec_dim=arr.shape[1])
 
     @staticmethod
+    def vector_int8(values: np.ndarray) -> "Column":
+        """VectorColumn::Int8((Buffer<i8>, dim)) (types/vector.rs:377-380).  The values must already be
+        int8: nothing is rounded or clipped here."""
+        arr = np.asarray(values)
+        if arr.dtype != np.int8 or arr.ndim != 2:
+            raise TypeError("Column.vector_int8 takes a 2-d int8 array")
+        arr = np.ascontiguousarray(arr)
+        return Column(abi.VEC_I8, arr.shape[0], data=arr, vec_dim=arr.shape[1])
+
+    @staticmethod
     def device(dtype: int, length: int, dev_ptr: int, vec_dim: int = 0, dev_validity: int = 0) -> "Column":
         return Column(dtype, length, dev_ptr=dev_ptr, vec_dim=vec_dim, dev_validity=dev_validity)
 
@@ -142,7 +153,7 @@ class Column:
         elif self.data is not None:
             c.data = self.data[start:end]
         else:
-            width = 4 * self.vec_dim if self.dtype == abi.VEC_F32 else np_dtype(self.dtype).itemsize
+            width = _VEC_ELEM[self.dtype].itemsize * self.vec_dim if self.dtype in _VEC_ELEM else np_dtype(self.dtype).itemsize
             c.dev_ptr = self.dev_ptr + start * width
         if self.validity is not None:
             c.validity = self.validity

@@ -6,7 +6,7 @@
 //   DataBlock::scatter(indices, n)        scatter.rs:21        (row i goes to block indices[i], order kept)
 //   DataBlock::concat(blocks)             concat.rs:62
 // Every column kind libdbx carries is handled: numeric Buffer<T>, Boolean (bit-packed), Vector(Float32)
-// (flat row-major), Nullable (validity Bitmap with a bit offset), BlockEntry::Const (stays const).
+// and Vector(Int8) (flat row-major), Nullable (validity Bitmap with a bit offset), BlockEntry::Const (stays const).
 // HBM-bound byte moving: one thread per output row and column element, coalesced on the output side.
 #include <algorithm>
 #include <vector>
@@ -23,7 +23,7 @@ struct GatherCol {
   int64_t src_vbit_off, src_dbit_off;
   void* dst;                  // values (BOOL: one byte per row, packed afterwards)
   uint8_t* dst_valid;         // one byte per row or nullptr
-  int32_t elt;                // bytes per row (vectors: 4 * dim); 0 = BOOL
+  int32_t elt;                // bytes per row (vectors: 4 * dim or dim); 0 = BOOL
   int32_t pad;
 };
 struct GatherParams {
@@ -47,10 +47,14 @@ __global__ void __launch_bounds__(256) gather_rows_kernel(const __grid_constant_
       else if (gc.elt == 4) ((uint32_t*)gc.dst)[o] = ((const uint32_t*)gc.src)[r];
       else if (gc.elt == 2) ((uint16_t*)gc.dst)[o] = ((const uint16_t*)gc.src)[r];
       else if (gc.elt == 1) ((uint8_t*)gc.dst)[o] = ((const uint8_t*)gc.src)[r];
-      else {  // Vector(Float32): elt = 4 * dim
+      else if ((gc.elt & 3) == 0) {  // Vector(Float32), or Vector(Int8) whose dim is a multiple of 4
         const uint32_t* s = (const uint32_t*)((const char*)gc.src + r * gc.elt);
         uint32_t* d = (uint32_t*)((char*)gc.dst + o * gc.elt);
         for (int k = 0; k < gc.elt / 4; ++k) d[k] = s[k];
+      } else {  // Vector(Int8) of any other dim
+        const uint8_t* s = (const uint8_t*)gc.src + r * gc.elt;
+        uint8_t* d = (uint8_t*)gc.dst + o * gc.elt;
+        for (int k = 0; k < gc.elt; ++k) d[k] = s[k];
       }
       if (gc.dst_valid) gc.dst_valid[o] = gc.src_valid ? (uint8_t)bit_test(gc.src_valid, gc.src_vbit_off + r) : 1;
     }
@@ -107,7 +111,7 @@ struct DeviceView {
       if (col.len != b->num_rows) { err.set("block kernel: column length differs from num_rows"); return DBX_ERR_INVALID; }
       if (col.is_const) { dc.is_const = 1; continue; }
       const bool is_bool = col.dtype == DBX_BOOL;
-      const int64_t elt = col.dtype == DBX_VEC_F32 ? 4LL * col.vec_dim : dtype_size(col.dtype);
+      const int64_t elt = column_row_bytes(col.dtype, col.vec_dim);
       if (!is_bool && elt == 0) { err.set("block kernel: unsupported column type"); return DBX_ERR_UNSUPPORTED; }
       if (col.mem == DBX_MEM_DEVICE) {
         dc.data = col.data; dc.validity = col.validity; dc.vbit_off = col.validity_bit_offset; dc.dbit_off = col.data_bit_offset;
@@ -152,7 +156,7 @@ struct OutputBuilder {
       memset(&oc, 0, sizeof(oc));
       oc.dtype = pc.dtype; oc.vec_dim = pc.vec_dim; oc.len = n_out; oc.mem = DBX_MEM_DEVICE;
       if (pc.is_const) { oc.is_const = 1; oc.konst = pc.konst; oc.mem = DBX_MEM_HOST; ob->cols.push_back(oc); continue; }
-      const int64_t elt = pc.dtype == DBX_BOOL ? 1 : (pc.dtype == DBX_VEC_F32 ? 4LL * pc.vec_dim : dtype_size(pc.dtype));
+      const int64_t elt = pc.dtype == DBX_BOOL ? 1 : column_row_bytes(pc.dtype, pc.vec_dim);
       void* d = nullptr;
       DBX_CUDA_TRY(err, pool_alloc(device, st, (size_t)std::max<int64_t>(n_out * elt, 1), &d));
       ob->dev_allocs.push_back(d);
@@ -180,7 +184,7 @@ struct OutputBuilder {
       gc.src = dc.data; gc.src_valid = dc.validity; gc.src_vbit_off = dc.vbit_off; gc.src_dbit_off = dc.dbit_off;
       gc.dst = (void*)ob->cols[(size_t)c].data;
       gc.dst_valid = valid_bytes[(size_t)c];
-      gc.elt = proto->cols[c].dtype == DBX_BOOL ? 0 : (proto->cols[c].dtype == DBX_VEC_F32 ? 4 * proto->cols[c].vec_dim : dtype_size(proto->cols[c].dtype));
+      gc.elt = (int32_t)column_row_bytes(proto->cols[c].dtype, proto->cols[c].vec_dim);
     }
     gp->n_cols = k;
   }
@@ -375,7 +379,7 @@ int32_t dbx_block_concat(int32_t device, const dbx_block* blocks, int32_t n_bloc
     total += blocks[b].num_rows;
   }
   for (int c = 0; c < first->num_cols; ++c)
-    if (!all_const[c] && first->cols[c].dtype == DBX_VEC_F32)
+    if (!all_const[c] && is_vector_dtype(first->cols[c].dtype))
       for (int b = 0; b < n_blocks; ++b)
         if (blocks[b].cols[c].is_const) { err.set("dbx_block_concat: constant vector columns cannot be materialised"); return DBX_ERR_UNSUPPORTED; }
   CallCtx cx;

@@ -68,6 +68,11 @@ __host__ __device__ inline int dtype_size(int dt) {
     default: return 0;
   }
 }
+// bytes of one row of a column: vectors are dim elements wide; 0 for BOOL (bit-packed)
+__host__ __device__ inline int64_t column_row_bytes(int dt, int vec_dim) {
+  return dt == DBX_VEC_F32 ? 4LL * vec_dim : dt == DBX_VEC_I8 ? (int64_t)vec_dim : (int64_t)dtype_size(dt);
+}
+__host__ __device__ inline bool is_vector_dtype(int dt) { return dt == DBX_VEC_F32 || dt == DBX_VEC_I8; }
 enum ValClass : int { VC_INT = 0, VC_UINT = 1, VC_FLT = 2 };
 __host__ __device__ inline int dtype_class(int dt) {
   switch (dt) {

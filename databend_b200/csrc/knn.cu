@@ -17,6 +17,9 @@
 //   4. the surviving k' candidates per query are re-evaluated EXACTLY in f32 with the reference's
 //      evaluation order and sorted by (distance, row id): returned distances are bit-identical to
 //      the row-wise function, the bf16 GEMM only decides which rows get that far.
+// A Vector(Int8) corpus takes the same plan with an int8 operand (no bf16 copy) and the s8 wgmma:
+// its dot products and norms are exact integers, so the only error left between the GEMM's score
+// and the reference distance is the f32 evaluation of the score itself.
 #include <cuda.h>
 
 #include <algorithm>
@@ -118,7 +121,8 @@ __device__ __forceinline__ uint32_t dist_to_ordered32(float d) {  // OrderedFloa
   const uint32_t b = __float_as_uint(d);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
-__global__ void rerank_kernel(int kind, const float* queries, const float* corpus, int dim, const uint64_t* keys,
+template <typename T>
+__global__ void rerank_kernel(int kind, const T* queries, const T* corpus, int dim, const uint64_t* keys,
                               const uint32_t* rows, int64_t n, uint64_t* out_keys, float* out_dist) {
   if (kind == DBX_DIST_COSINE) {
     const int lane = threadIdx.x & 31, g = lane >> 3;
@@ -167,6 +171,22 @@ __global__ void rerank_kernel(int kind, const float* queries, const float* corpu
 // The constants are computed for the corpus's dim on the host (certificate_constants).  The budget
 // holds for rows whose squared norms are in range (prep_rows_kernel): a query out of range, or a
 // corpus with a row out of range that is not NaN for every query, is answered exactly.
+//
+// Int8 corpora (s8 wgmma, exact int32 accumulators, prep_rows_i8_kernel, i8_score): the bf16,
+// accumulator and normalisation terms are gone — ab, |q|^2 and |c|^2 are exact integers.  Left:
+//  * cosine: the score (f32(ab) * 1/|q|) * 1/|c| — f32(ab) 2^-24, each reciprocal norm from an
+//    f32-rounded sum, an f32 sqrt and an f32 division <= 2.5 2^-24, two multiplies 2 2^-24 —
+//    is within 8 2^-24 of the similarity (|similarity| <= 1); the budget takes 16 2^-24, plus the
+//    reference's f32 evaluation (`exact` above) and the 32 2^-24 compare term;
+//  * L2: the score -S is exact before its one rounding to f32, 2^-24 S <= 2^-23 (|q|^2 + |c|^2);
+//    |q|^2 and cmax^2 in the certificate are themselves f32-rounded (a few 2^-24), and so is the
+//    compare: l2_norms = 2^-21 covers all of it, l2_cross = 0; l2_rel and l2_floor as above.
+// int8 has no inf or NaN, so no row is outside the range (corpus_unsafe = 0); zero rows are NaN
+// for every query under cosine and harmless, as above.  Every term stays strictly positive even
+// where the score is exact: with int8 data exact ties in distance are ordinary (duplicate rows, or
+// distinct integer similarities that round to one f32 distance), the cut keeps tied rows in an
+// arbitrary order, and only a positive margin sends a tie at the boundary to the exact path instead
+// of returning a higher row id.
 struct KnnCertificate {
   float cos_margin;  // cosine: certified iff 1 - d_k >= bound + cos_margin
   float l2_cross;    // L2: e = l2_cross |q| cmax + l2_norms (|q|^2 + cmax^2) + l2_floor (1 + |q|)
@@ -200,13 +220,24 @@ __global__ void certify_kernel(int kind, int nq, int k, int kk, const int64_t* s
     flags[q] = ok ? 0 : 1;
   }
 }
-KnnCertificate certificate_constants(int kind, int dim, int corpus_unsafe) {
+KnnCertificate certificate_constants(int kind, int dim, int corpus_unsafe, bool int8) {
   const double n = dim, f32 = std::ldexp(1.0, -24), u = std::ldexp(1.0, -8);
   const double bf16 = (1.0 + u / (1.0 + u)) * (1.0 + u / (1.0 + u)) - 1.0;  // 0.0077972
   const double acc = 2.0 * n * std::ldexp(1.0, -23) * 1.008;
   KnnCertificate c;
   memset(&c, 0, sizeof(c));
   c.corpus_unsafe = corpus_unsafe;
+  if (int8) {
+    if (kind == DBX_DIST_COSINE) {
+      const double exact = (2.0 * (n / 8 + 13) + 4) * f32;
+      c.cos_margin = (float)(16 * f32 + exact + 32 * f32);
+    } else {
+      c.l2_norms = (float)std::ldexp(1.0, -21);
+      c.l2_floor = (float)(n * std::ldexp(1.0, -120));
+      c.l2_rel = (float)((n + 16) * std::ldexp(1.0, -23));
+    }
+    return c;
+  }
   if (kind == DBX_DIST_COSINE) {
     const double norm = std::ldexp(1.0, -21) + (n / 32 + 8) * f32;
     const double exact = (2.0 * (n / 8 + 13) + 4) * f32;
@@ -444,15 +475,17 @@ PFN_encodeTiled get_encode_fn() {
   }
   return fn;
 }
-// bf16 matrix [rows, dim_pad] row-major, box = [64 (K), box_rows], 128-byte swizzle
-bool make_tmap(CUtensorMap* m, const void* base, int64_t rows, int dim_pad, int box_rows) {
+// bf16 / int8 matrix [rows, dim_pad] row-major, box = [one 128-byte k-block, box_rows], 128-byte
+// swizzle.  int8 is described as UINT8 (there is no signed 8-bit tensor-map type; TMA moves bytes).
+bool make_tmap(CUtensorMap* m, const void* base, int64_t rows, int dim_pad, int box_rows, bool int8) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) return false;
+  const int es = int8 ? 1 : 2;
   cuuint64_t dims[2] = {(cuuint64_t)dim_pad, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)dim_pad * 2};
-  cuuint32_t box[2] = {(cuuint32_t)kGemmBK, (cuuint32_t)box_rows};
+  cuuint64_t strides[1] = {(cuuint64_t)dim_pad * es};
+  cuuint32_t box[2] = {(cuuint32_t)(kKBlockBytes / es), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+  return enc(m, int8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
@@ -467,13 +500,14 @@ struct dbx_knn {
   ErrorSink err;
   int device = 0;
   int kind = 0;
+  bool int8 = false;  // Vector(Int8) corpus: int8 operands, s8 wgmma; else Vector(Float32), bf16 operands
   int dim = 0, dim_pad = 0;
   int64_t n = 0;
   cudaStream_t stream = nullptr;
-  const float* corpus = nullptr;  // f32 [n, dim] in HBM (borrowed if the caller passed device memory)
-  DevBuf corpus_own, corpus_bf16, c_scale;
+  const void* corpus = nullptr;  // f32 / i8 [n, dim] in HBM (borrowed if the caller passed device memory)
+  DevBuf corpus_own, corpus_op, c_scale, c_sq;  // corpus_op: the GEMM operand (bf16 or int8, [n + 128, dim_pad])
   // per-search scratch (grow-only)
-  DevBuf q_f32, q_bf16, q_scale, bound, seg, seg_off, cand_key[2], cand_row[2], counters, perm[2], key_tmp, sort_alt, dist, qcount;
+  DevBuf q_raw, q_op, q_scale, q_sq, bound, seg, seg_off, cand_key[2], cand_row[2], counters, perm[2], key_tmp, sort_alt, dist, qcount;
   DevBuf out_idx_dev, out_dist_dev, max_norm, flags, ex_dist, ex_key[2], ex_row[2], ex_tmp;
   PinnedBuf host, host_flags;
   int corpus_unsafe = 0;  // rows outside the certificate's norm range (prep_rows_kernel)
@@ -487,13 +521,13 @@ struct dbx_knn {
   ~dbx_knn() { for (cudaEvent_t e : pass_ev) cudaEventDestroy(e); }
 };
 
-// Launch plumbing of the similarity GEMM for a cluster size C in {1,2,4,8}.
-template <int C>
+// Launch plumbing of the similarity GEMM for a cluster size C in {1,2,4,8} and operand type T.
+template <int C, typename T>
 static int32_t gemm_prepare_t(ErrorSink& err, int* max_clusters) {
   static int cached = -1;
   if (cached < 0) {
     const int smem = (int)(sizeof(GemmSmem) + 1024);
-    DBX_CUDA_TRY(err, cudaFuncSetAttribute(knn_gemm_filter_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DBX_CUDA_TRY(err, cudaFuncSetAttribute(knn_gemm_filter_kernel<C, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int n = kNumSMs / C;
     if (C > 1) {
       cudaLaunchConfig_t cfg;
@@ -506,7 +540,7 @@ static int32_t gemm_prepare_t(ErrorSink& err, int* max_clusters) {
       at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
       cfg.attrs = at; cfg.numAttrs = 1;
       int q = 0;
-      DBX_CUDA_TRY(err, cudaOccupancyMaxActiveClusters(&q, knn_gemm_filter_kernel<C>, &cfg));
+      DBX_CUDA_TRY(err, cudaOccupancyMaxActiveClusters(&q, knn_gemm_filter_kernel<C, T>, &cfg));
       if (q < 1) { err.set("similarity GEMM: no co-resident cluster fits on this device"); return DBX_ERR_CUDA; }
       n = std::min(n, q);
     }
@@ -515,7 +549,7 @@ static int32_t gemm_prepare_t(ErrorSink& err, int* max_clusters) {
   *max_clusters = cached;
   return DBX_OK;
 }
-template <int C>
+template <int C, typename T>
 static int32_t gemm_launch_t(ErrorSink& err, int n_clusters, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tc, const KnnGemmParams& gp) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -527,25 +561,35 @@ static int32_t gemm_launch_t(ErrorSink& err, int n_clusters, cudaStream_t st, co
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
-  DBX_CUDA_TRY(err, cudaLaunchKernelEx(&cfg, knn_gemm_filter_kernel<C>, tq, tc, gp));
+  DBX_CUDA_TRY(err, cudaLaunchKernelEx(&cfg, knn_gemm_filter_kernel<C, T>, tq, tc, gp));
   return DBX_OK;
 }
-static int32_t knn_gemm_prepare(ErrorSink& err, int cluster, int* max_clusters) {
+template <typename T>
+static int32_t knn_gemm_prepare_t(ErrorSink& err, int cluster, int* max_clusters) {
   switch (cluster) {
-    case 1: return gemm_prepare_t<1>(err, max_clusters);
-    case 2: return gemm_prepare_t<2>(err, max_clusters);
-    case 4: return gemm_prepare_t<4>(err, max_clusters);
-    default: return gemm_prepare_t<8>(err, max_clusters);
+    case 1: return gemm_prepare_t<1, T>(err, max_clusters);
+    case 2: return gemm_prepare_t<2, T>(err, max_clusters);
+    case 4: return gemm_prepare_t<4, T>(err, max_clusters);
+    default: return gemm_prepare_t<8, T>(err, max_clusters);
   }
 }
-static int32_t knn_gemm_launch(ErrorSink& err, int cluster, int n_clusters, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tc,
-                               const KnnGemmParams& gp) {
+template <typename T>
+static int32_t knn_gemm_launch_t(ErrorSink& err, int cluster, int n_clusters, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tc,
+                                 const KnnGemmParams& gp) {
   switch (cluster) {
-    case 1: return gemm_launch_t<1>(err, n_clusters, st, tq, tc, gp);
-    case 2: return gemm_launch_t<2>(err, n_clusters, st, tq, tc, gp);
-    case 4: return gemm_launch_t<4>(err, n_clusters, st, tq, tc, gp);
-    default: return gemm_launch_t<8>(err, n_clusters, st, tq, tc, gp);
+    case 1: return gemm_launch_t<1, T>(err, n_clusters, st, tq, tc, gp);
+    case 2: return gemm_launch_t<2, T>(err, n_clusters, st, tq, tc, gp);
+    case 4: return gemm_launch_t<4, T>(err, n_clusters, st, tq, tc, gp);
+    default: return gemm_launch_t<8, T>(err, n_clusters, st, tq, tc, gp);
   }
+}
+static int32_t knn_gemm_prepare(ErrorSink& err, bool int8, int cluster, int* max_clusters) {
+  return int8 ? knn_gemm_prepare_t<int8_t>(err, cluster, max_clusters) : knn_gemm_prepare_t<__nv_bfloat16>(err, cluster, max_clusters);
+}
+static int32_t knn_gemm_launch(ErrorSink& err, bool int8, int cluster, int n_clusters, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tc,
+                               const KnnGemmParams& gp) {
+  return int8 ? knn_gemm_launch_t<int8_t>(err, cluster, n_clusters, st, tq, tc, gp)
+              : knn_gemm_launch_t<__nv_bfloat16>(err, cluster, n_clusters, st, tq, tc, gp);
 }
 
 // Exact answer for one query: distance to every corpus row (row-wise kernel, reference evaluation
@@ -563,8 +607,13 @@ static int32_t knn_exact_query(dbx_knn* h, int q, int k, int kk) {
       DBX_CUDA_TRY(err, h->ex_key[i].ensure((size_t)n * 8));
       DBX_CUDA_TRY(err, h->ex_row[i].ensure((size_t)n * 4));
     }
-    distance_rows_kernel<<<grid_1d(h->kind == DBX_DIST_COSINE ? n * 8 : n, 128), 128, 0, st>>>(
-        h->kind, h->corpus, 0, (const float*)h->q_f32.p + (int64_t)q * h->dim, 1, n, h->dim, nullptr, 0, nullptr, 0, (float*)h->ex_dist.p, nullptr);
+    const int grid = grid_1d(h->kind == DBX_DIST_COSINE ? n * 8 : n, 128);
+    if (h->int8)
+      distance_rows_kernel<<<grid, 128, 0, st>>>(h->kind, (const int8_t*)h->corpus, 0, (const int8_t*)h->q_raw.p + (int64_t)q * h->dim, 1, n, h->dim,
+                                                 nullptr, 0, nullptr, 0, (float*)h->ex_dist.p, nullptr);
+    else
+      distance_rows_kernel<<<grid, 128, 0, st>>>(h->kind, (const float*)h->corpus, 0, (const float*)h->q_raw.p + (int64_t)q * h->dim, 1, n, h->dim,
+                                                 nullptr, 0, nullptr, 0, (float*)h->ex_dist.p, nullptr);
     exact_keys_kernel<<<grid_1d(n), 256, 0, st>>>((const float*)h->ex_dist.p, n, (uint64_t*)h->ex_key[0].p, (uint32_t*)h->ex_row[0].p);
     // stable LSD radix sort on the 32 significant key bits: ties keep ascending row ids
     DBX_TRY(h->sorter.sort(err, st, (uint64_t*)h->ex_key[0].p, (uint64_t*)h->ex_key[1].p, (uint32_t*)h->ex_row[0].p, (uint32_t*)h->ex_row[1].p, n, 0, 32,
@@ -585,38 +634,55 @@ int32_t dbx_knn_create(int32_t kind, int32_t device, const dbx_column* corpus, d
   if (!corpus || !out) { g_create_error.set("dbx_knn_create: null argument"); return DBX_ERR_INVALID; }
   *out = nullptr;
   if (kind != DBX_DIST_COSINE && kind != DBX_DIST_L2) { g_create_error.set("dbx_knn_create: unknown distance kind"); return DBX_ERR_INVALID; }
-  if (corpus->dtype != DBX_VEC_F32 || corpus->vec_dim <= 0) { g_create_error.set("dbx_knn_create: corpus must be a VECTOR(Float32) column"); return DBX_ERR_INVALID; }
+  if ((corpus->dtype != DBX_VEC_F32 && corpus->dtype != DBX_VEC_I8) || corpus->vec_dim <= 0) {
+    g_create_error.set("dbx_knn_create: corpus must be a VECTOR(Float32) or VECTOR(Int8) column");
+    return DBX_ERR_INVALID;
+  }
+  if (corpus->dtype == DBX_VEC_I8 && corpus->vec_dim >= 131072) {  // the s8 wgmma's int32 accumulators hold |sum ab| < 2^31
+    g_create_error.set("dbx_knn_create: VECTOR(Int8) corpora are limited to dim < 131072");
+    return DBX_ERR_UNSUPPORTED;
+  }
   if (corpus->validity) { g_create_error.set("dbx_knn_create: NULL vectors in the corpus are not supported yet"); return DBX_ERR_UNSUPPORTED; }
   if (corpus->len >= (1LL << 31)) { g_create_error.set("dbx_knn_create: corpus too large for 32-bit row ids"); return DBX_ERR_UNSUPPORTED; }
   int32_t ndev = 0;
   DBX_TRY(dbx_device_count(&ndev));
   std::unique_ptr<dbx_knn> h(new dbx_knn());
   ErrorSink& err = g_create_error;
-  h->device = device; h->kind = kind; h->dim = corpus->vec_dim; h->dim_pad = round_up(corpus->vec_dim, kGemmBK); h->n = corpus->len;
+  h->device = device; h->kind = kind; h->int8 = corpus->dtype == DBX_VEC_I8; h->dim = corpus->vec_dim; h->n = corpus->len;
+  h->dim_pad = round_up(corpus->vec_dim, h->int8 ? kBlockK<int8_t> : kBlockK<__nv_bfloat16>);
+  const int es = h->int8 ? 1 : 4, op_es = h->int8 ? 1 : 2;  // bytes per element of the corpus / of the GEMM operand
   DBX_CUDA_TRY(err, cudaSetDevice(device));
   DBX_CUDA_TRY(err, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   DBX_CUDA_TRY(err, cudaEventCreate(&h->ev0));
   DBX_CUDA_TRY(err, cudaEventCreate(&h->ev1));
-  const size_t bytes = (size_t)h->n * h->dim * 4;
+  const size_t bytes = (size_t)h->n * h->dim * es;
   if (corpus->mem == DBX_MEM_DEVICE) {
-    h->corpus = (const float*)corpus->data;
+    h->corpus = corpus->data;
   } else {
     DBX_CUDA_TRY(err, h->corpus_own.ensure(bytes ? bytes : 4));
     DBX_CUDA_TRY(err, cudaMemcpyAsync(h->corpus_own.p, corpus->data, bytes, cudaMemcpyHostToDevice, h->stream));
-    h->corpus = (const float*)h->corpus_own.p;
+    h->corpus = h->corpus_own.p;
   }
-  // the bf16 copy is padded by one GEMM tile of rows so that every TMA box stays inside the tensor
+  // the operand copy is padded by one GEMM tile of rows so that every TMA box stays inside the tensor
   const int64_t n_alloc = h->n + kGemmBN;
-  DBX_CUDA_TRY(err, h->corpus_bf16.ensure((size_t)n_alloc * h->dim_pad * 2));
-  DBX_CUDA_TRY(err, cudaMemsetAsync(h->corpus_bf16.p, 0, (size_t)n_alloc * h->dim_pad * 2, h->stream));
+  DBX_CUDA_TRY(err, h->corpus_op.ensure((size_t)n_alloc * h->dim_pad * op_es));
+  DBX_CUDA_TRY(err, cudaMemsetAsync(h->corpus_op.p, 0, (size_t)n_alloc * h->dim_pad * op_es, h->stream));
   DBX_CUDA_TRY(err, h->c_scale.ensure((size_t)n_alloc * 4));
   DBX_CUDA_TRY(err, cudaMemsetAsync(h->c_scale.p, 0, (size_t)n_alloc * 4, h->stream));
+  if (h->int8) {
+    DBX_CUDA_TRY(err, h->c_sq.ensure((size_t)n_alloc * 4));
+    DBX_CUDA_TRY(err, cudaMemsetAsync(h->c_sq.p, 0, (size_t)n_alloc * 4, h->stream));
+  }
   DBX_CUDA_TRY(err, h->max_norm.ensure(8));  // [0] largest row norm (bits), [1] rows outside the certificate's range
   DBX_CUDA_TRY(err, cudaMemsetAsync(h->max_norm.p, 0, 8, h->stream));
   if (h->n) {
-    prep_rows_kernel<<<grid_1d(h->n * 32), 256, 0, h->stream>>>(h->corpus, h->n, h->dim, h->dim_pad, (__nv_bfloat16*)h->corpus_bf16.p,
-                                                              (float*)h->c_scale.p, kind, (unsigned int*)h->max_norm.p,
-                                                              (unsigned int*)h->max_norm.p + 1);
+    if (h->int8)
+      prep_rows_i8_kernel<<<grid_1d(h->n * 32), 256, 0, h->stream>>>((const int8_t*)h->corpus, h->n, h->dim, h->dim_pad, (int8_t*)h->corpus_op.p,
+                                                                   (int32_t*)h->c_sq.p, (float*)h->c_scale.p, kind, (unsigned int*)h->max_norm.p);
+    else
+      prep_rows_kernel<<<grid_1d(h->n * 32), 256, 0, h->stream>>>((const float*)h->corpus, h->n, h->dim, h->dim_pad, (__nv_bfloat16*)h->corpus_op.p,
+                                                                (float*)h->c_scale.p, kind, (unsigned int*)h->max_norm.p,
+                                                                (unsigned int*)h->max_norm.p + 1);
     count_launch();
     DBX_CUDA_TRY(err, cudaGetLastError());
   }
@@ -650,7 +716,12 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   if (!h) return DBX_ERR_INVALID;
   ErrorSink& err = h->err;
   if (!queries || !out_idx || !out_dist || k <= 0) { err.set("dbx_knn_search: bad argument"); return DBX_ERR_INVALID; }
-  if (queries->dtype != DBX_VEC_F32 || queries->vec_dim != h->dim) { err.set("Vector length not equal: query dimension differs from the corpus"); return DBX_ERR_INVALID; }
+  if (queries->dtype != (h->int8 ? DBX_VEC_I8 : DBX_VEC_F32)) {
+    // the reference would answer 0.0 (or NULL) on every row of a mixed Int8 / Float32 pair
+    err.set(h->int8 ? "dbx_knn_search: queries must be VECTOR(Int8) like the corpus" : "dbx_knn_search: queries must be VECTOR(Float32) like the corpus");
+    return DBX_ERR_INVALID;
+  }
+  if (queries->vec_dim != h->dim) { err.set("Vector length not equal: query dimension differs from the corpus"); return DBX_ERR_INVALID; }
   if (queries->validity) { err.set("dbx_knn_search: NULL query vectors are not supported yet"); return DBX_ERR_UNSUPPORTED; }
   if (k > 1024) { err.set("dbx_knn_search: k > 1024 is not supported"); return DBX_ERR_UNSUPPORTED; }
   DBX_CUDA_TRY(err, cudaSetDevice(h->device));
@@ -673,18 +744,25 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   const int dim = h->dim, dim_pad = h->dim_pad;
   const int kprime = round_up(std::max(8 * k, 64), 64);
 
-  // ---- queries: f32 (exact re-rank) + bf16 + scale
-  DBX_CUDA_TRY(err, h->q_f32.ensure((size_t)nq_pad * dim * 4));
-  DBX_CUDA_TRY(err, h->q_bf16.ensure((size_t)nq_pad * dim_pad * 2));
+  // ---- queries: f32 / i8 as given (exact re-rank) + GEMM operand (bf16 / int8) + scale
+  const int es = h->int8 ? 1 : 4, op_es = h->int8 ? 1 : 2;
+  DBX_CUDA_TRY(err, h->q_raw.ensure((size_t)nq_pad * dim * es));
+  DBX_CUDA_TRY(err, h->q_op.ensure((size_t)nq_pad * dim_pad * op_es));
   DBX_CUDA_TRY(err, h->q_scale.ensure((size_t)nq_pad * 4));
   DBX_CUDA_TRY(err, h->bound.ensure((size_t)nq_pad * 4));
   DBX_CUDA_TRY(err, h->seg.ensure((size_t)(nq + 2) * 8));
   DBX_CUDA_TRY(err, h->seg_off.ensure((size_t)(nq + 2) * 8));
-  DBX_CUDA_TRY(err, cudaMemsetAsync(h->q_f32.p, 0, (size_t)nq_pad * dim * 4, st));
-  DBX_CUDA_TRY(err, cudaMemcpyAsync(h->q_f32.p, queries->data, (size_t)nq * dim * 4,
+  DBX_CUDA_TRY(err, cudaMemsetAsync(h->q_raw.p, 0, (size_t)nq_pad * dim * es, st));
+  DBX_CUDA_TRY(err, cudaMemcpyAsync(h->q_raw.p, queries->data, (size_t)nq * dim * es,
                                     queries->mem == DBX_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-  prep_rows_kernel<<<grid_1d((int64_t)nq_pad * 32), 256, 0, st>>>((const float*)h->q_f32.p, nq_pad, dim, dim_pad, (__nv_bfloat16*)h->q_bf16.p,
-                                                                (float*)h->q_scale.p, h->kind, nullptr, nullptr);
+  if (h->int8) {
+    DBX_CUDA_TRY(err, h->q_sq.ensure((size_t)nq_pad * 4));
+    prep_rows_i8_kernel<<<grid_1d((int64_t)nq_pad * 32), 256, 0, st>>>((const int8_t*)h->q_raw.p, nq_pad, dim, dim_pad, (int8_t*)h->q_op.p,
+                                                                     (int32_t*)h->q_sq.p, (float*)h->q_scale.p, h->kind, nullptr);
+  } else {
+    prep_rows_kernel<<<grid_1d((int64_t)nq_pad * 32), 256, 0, st>>>((const float*)h->q_raw.p, nq_pad, dim, dim_pad, (__nv_bfloat16*)h->q_op.p,
+                                                                  (float*)h->q_scale.p, h->kind, nullptr, nullptr);
+  }
   count_launch();
 
   // ---- candidate storage
@@ -772,12 +850,12 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   const bool use_ref = getenv("DBX_KNN_REF_GEMM") != nullptr;
   int max_clusters = kNumSMs / cluster;
   if (!use_ref) {
-    if (!make_tmap(&tmap_q, h->q_bf16.p, nq_pad, dim_pad, kGemmBM) ||
-        !make_tmap(&tmap_c, h->corpus_bf16.p, h->n + kGemmBN, dim_pad, kGemmBN / cluster)) {
+    if (!make_tmap(&tmap_q, h->q_op.p, nq_pad, dim_pad, kGemmBM, h->int8) ||
+        !make_tmap(&tmap_c, h->corpus_op.p, h->n + kGemmBN, dim_pad, kGemmBN / cluster, h->int8)) {
       err.set("cuTensorMapEncodeTiled failed (TMA descriptors for the similarity GEMM)");
       return DBX_ERR_CUDA;
     }
-    DBX_TRY(knn_gemm_prepare(err, cluster, &max_clusters));
+    DBX_TRY(knn_gemm_prepare(err, h->int8, cluster, &max_clusters));
     h->stat_cluster = cluster; h->stat_grid = (int64_t)max_clusters * cluster;
   }
   for (int attempt = 0; attempt < 2; ++attempt) {
@@ -801,6 +879,7 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
       gp.kind = h->kind; gp.nq = nq; gp.nq_pad = nq_pad; gp.dim_pad = dim_pad; gp.n0 = done; gp.n_rows = m;
       gp.q_scale = (const float*)h->q_scale.p; gp.c_scale = (const float*)h->c_scale.p; gp.bound = (const float*)h->bound.p;
       gp.cand_key = (uint64_t*)h->cand_key[perq ? 1 : cur].p; gp.cand_row = (uint32_t*)h->cand_row[perq ? 1 : cur].p; gp.cand_count = d_count; gp.cand_cap = cap;
+      gp.q_sq = (const int32_t*)h->q_sq.p; gp.c_sq = (const int32_t*)h->c_sq.p;
       cudaEvent_t e0 = h->ev0, e1 = h->ev1;
       if (async_mode) {
         if (!perq) DBX_CUDA_TRY(err, cudaMemcpyAsync(d_prev, d_count, 8, cudaMemcpyDeviceToDevice, st));
@@ -813,12 +892,14 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
         n_ev += 2;
       }
       DBX_CUDA_TRY(err, cudaEventRecord(e0, st));
-      if (use_ref) {
-        knn_ref_filter_kernel<<<grid_1d((int64_t)nq * m), 256, 0, st>>>((const __nv_bfloat16*)h->q_bf16.p, (const __nv_bfloat16*)h->corpus_bf16.p, gp);
+      if (use_ref && h->int8) {
+        knn_ref_filter_i8_kernel<<<grid_1d((int64_t)nq * m), 256, 0, st>>>((const int8_t*)h->q_op.p, (const int8_t*)h->corpus_op.p, gp);
+      } else if (use_ref) {
+        knn_ref_filter_kernel<<<grid_1d((int64_t)nq * m), 256, 0, st>>>((const __nv_bfloat16*)h->q_op.p, (const __nv_bfloat16*)h->corpus_op.p, gp);
       } else {
         const int64_t tiles = ((m + kGemmBN - 1) / kGemmBN) * (nq_pad / (kGemmBM * cluster));
         const int n_clusters = (int)std::min<int64_t>(tiles, max_clusters);
-        DBX_TRY(knn_gemm_launch(err, cluster, n_clusters, st, tmap_q, tmap_c, gp));
+        DBX_TRY(knn_gemm_launch(err, h->int8, cluster, n_clusters, st, tmap_q, tmap_c, gp));
       }
       count_launch();
       DBX_CUDA_TRY(err, cudaGetLastError());
@@ -886,8 +967,12 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   if (n_cand > 0) {
     // exact distances, then two stable LSD radix sorts of a permutation: by row id, then by
     // (query, exact distance) -> ties keep ascending row ids
-    rerank_kernel<<<grid_1d(n_cand), 256, 0, st>>>(h->kind, (const float*)h->q_f32.p, h->corpus, dim, (const uint64_t*)h->cand_key[cur].p,
-                                                   (const uint32_t*)h->cand_row[cur].p, n_cand, (uint64_t*)h->key_tmp.p, (float*)h->dist.p);
+    if (h->int8)
+      rerank_kernel<<<grid_1d(n_cand), 256, 0, st>>>(h->kind, (const int8_t*)h->q_raw.p, (const int8_t*)h->corpus, dim, (const uint64_t*)h->cand_key[cur].p,
+                                                     (const uint32_t*)h->cand_row[cur].p, n_cand, (uint64_t*)h->key_tmp.p, (float*)h->dist.p);
+    else
+      rerank_kernel<<<grid_1d(n_cand), 256, 0, st>>>(h->kind, (const float*)h->q_raw.p, (const float*)h->corpus, dim, (const uint64_t*)h->cand_key[cur].p,
+                                                     (const uint32_t*)h->cand_row[cur].p, n_cand, (uint64_t*)h->key_tmp.p, (float*)h->dist.p);
     iota32_kernel<<<grid_1d(n_cand), 256, 0, st>>>((uint32_t*)h->perm[0].p, n_cand);
     uint64_t* ka = (uint64_t*)h->cand_key[cur ^ 1].p;
     uint64_t* kb = (uint64_t*)h->sort_alt.p;
@@ -919,7 +1004,7 @@ int32_t dbx_knn_search(dbx_knn* h, const dbx_column* queries, int32_t k, int32_t
   DBX_CUDA_TRY(err, h->host_flags.ensure((size_t)nq));
   certify_kernel<<<grid_1d(nq), 256, 0, st>>>(h->kind, nq, k, kk, (const int64_t*)h->seg.p, (const float*)h->bound.p, (const float*)h->q_scale.p,
                                              (const unsigned int*)h->max_norm.p, (const float*)h->out_dist_dev.p,
-                                             certificate_constants(h->kind, dim, h->corpus_unsafe), (uint8_t*)h->flags.p);
+                                             certificate_constants(h->kind, dim, h->corpus_unsafe, h->int8), (uint8_t*)h->flags.p);
   count_launch();
   DBX_CUDA_TRY(err, cudaGetLastError());
   DBX_CUDA_TRY(err, cudaMemcpyAsync(h->host_flags.p, h->flags.p, (size_t)nq, cudaMemcpyDeviceToHost, st));
@@ -957,8 +1042,15 @@ int32_t dbx_eval_distance(int32_t kind, int32_t device, const dbx_column* lhs, c
   ErrorSink& err = g_create_error;
   if (!lhs || !rhs || !out) { err.set("dbx_eval_distance: null argument"); return DBX_ERR_INVALID; }
   if (kind != DBX_DIST_COSINE && kind != DBX_DIST_L2) { err.set("dbx_eval_distance: unknown distance kind"); return DBX_ERR_INVALID; }
-  if (lhs->dtype != DBX_VEC_F32 || rhs->dtype != DBX_VEC_F32) { err.set("dbx_eval_distance: arguments must be VECTOR(Float32)"); return DBX_ERR_INVALID; }
-  if (lhs->vec_dim != rhs->vec_dim) {  // distance.rs:20-26
+  if (!is_vector_dtype(lhs->dtype) || !is_vector_dtype(rhs->dtype)) {
+    err.set("dbx_eval_distance: arguments must be VECTOR(Float32) or VECTOR(Int8)");
+    return DBX_ERR_INVALID;
+  }
+  // A Vector(Int8) / Vector(Float32) pair passes the reference's type check (dims are compared only
+  // for equal element types, scalars/vector.rs:458-494), then calculate_distance's `(_, _)` arm marks
+  // every row invalid and writes 0.0: 0.0 everywhere, NULL everywhere when the result is Nullable.
+  const bool mixed = lhs->dtype != rhs->dtype;
+  if (!mixed && lhs->vec_dim != rhs->vec_dim) {  // distance.rs:20-26
     err.set("Vector length not equal: " + std::to_string(lhs->vec_dim) + " != " + std::to_string(rhs->vec_dim));
     return DBX_ERR_INVALID;
   }
@@ -969,21 +1061,33 @@ int32_t dbx_eval_distance(int32_t kind, int32_t device, const dbx_column* lhs, c
   DBX_TRY(dbx_device_count(&ndev));
   DBX_CUDA_TRY(err, cudaSetDevice(device));
   if (rows == 0) return DBX_OK;
+  if (mixed) {
+    if (out->mem == DBX_MEM_DEVICE) DBX_CUDA_TRY(err, cudaMemset((void*)out->data, 0, (size_t)rows * 4));
+    else memset((void*)out->data, 0, (size_t)rows * 4);
+    if (out->validity) {
+      if (out->mem == DBX_MEM_DEVICE) DBX_CUDA_TRY(err, cudaMemset((void*)out->validity, 0, (size_t)(rows + 7) / 8));
+      else memset((void*)out->validity, 0, (size_t)(rows + 7) / 8);
+      out->null_count = rows;
+      out->validity_bit_offset = 0;
+    }
+    return DBX_OK;
+  }
   const int dim = lhs->vec_dim;
+  const int es = lhs->dtype == DBX_VEC_I8 ? 1 : 4;
   // const sides carry their single vector in `data` (len 1)
   DevBuf la, ra, lvb, rvb, ob, ovb, obits;
-  auto to_dev = [&](const dbx_column* c, DevBuf& buf, const float** p) -> int32_t {
-    const size_t bytes = (size_t)(c->is_const ? 1 : c->len) * dim * 4;
+  auto to_dev = [&](const dbx_column* c, DevBuf& buf, const void** p) -> int32_t {
+    const size_t bytes = (size_t)(c->is_const ? 1 : c->len) * dim * es;
     if (c->is_const && (c->konst.is_null || !c->data)) {  // NULL constant: every output row is NULL
       DBX_CUDA_TRY(err, buf.ensure(bytes));
       DBX_CUDA_TRY(err, cudaMemset(buf.p, 0, bytes));
-      *p = (const float*)buf.p;
+      *p = buf.p;
       return DBX_OK;
     }
-    if (c->mem == DBX_MEM_DEVICE) { *p = (const float*)c->data; return DBX_OK; }
+    if (c->mem == DBX_MEM_DEVICE) { *p = c->data; return DBX_OK; }
     DBX_CUDA_TRY(err, buf.ensure(bytes));
     DBX_CUDA_TRY(err, cudaMemcpy(buf.p, c->data, bytes, cudaMemcpyHostToDevice));
-    *p = (const float*)buf.p;
+    *p = buf.p;
     return DBX_OK;
   };
   auto valid_to_dev = [&](const dbx_column* c, DevBuf& buf, const uint8_t** p, int64_t* off) -> int32_t {
@@ -996,7 +1100,7 @@ int32_t dbx_eval_distance(int32_t kind, int32_t device, const dbx_column* lhs, c
     *p = (const uint8_t*)buf.p; *off = c->validity_bit_offset & 7;
     return DBX_OK;
   };
-  const float *lp, *rp;
+  const void *lp, *rp;
   const uint8_t *lv, *rv;
   int64_t lvo, rvo;
   DBX_TRY(to_dev(lhs, la, &lp));
@@ -1010,7 +1114,11 @@ int32_t dbx_eval_distance(int32_t kind, int32_t device, const dbx_column* lhs, c
   const bool want_valid = out->validity != nullptr;
   if (want_valid) { DBX_CUDA_TRY(err, ovb.ensure((size_t)rows)); ovalid = (uint8_t*)ovb.p; }
   if ((lv || rv || const_null) && !want_valid) { err.set("dbx_eval_distance: nullable inputs need out->validity"); return DBX_ERR_INVALID; }
-  distance_rows_kernel<<<grid_1d(kind == DBX_DIST_COSINE ? rows * 8 : rows, 128), 128>>>(kind, lp, lhs->is_const, rp, rhs->is_const, rows, dim, lv, lvo, rv, rvo, op, ovalid);
+  const int grid = grid_1d(kind == DBX_DIST_COSINE ? rows * 8 : rows, 128);
+  if (es == 1)
+    distance_rows_kernel<<<grid, 128>>>(kind, (const int8_t*)lp, lhs->is_const, (const int8_t*)rp, rhs->is_const, rows, dim, lv, lvo, rv, rvo, op, ovalid);
+  else
+    distance_rows_kernel<<<grid, 128>>>(kind, (const float*)lp, lhs->is_const, (const float*)rp, rhs->is_const, rows, dim, lv, lvo, rv, rvo, op, ovalid);
   count_launch();
   DBX_CUDA_TRY(err, cudaGetLastError());
   if (out->mem != DBX_MEM_DEVICE) DBX_CUDA_TRY(err, cudaMemcpy((void*)out->data, op, (size_t)rows * 4, cudaMemcpyDeviceToHost));

@@ -3,13 +3,17 @@
 //  (1) exact row-wise cosine / L2 in f32 with the reference's evaluation order
 //      (src/common/vector/src/distance.rs:19-35,65-80; ndarray 0.15.6 unrolled_fold for the
 //      cosine sums) — the ScalarFunction::eval replacement and the re-rank of kNN candidates;
+//      templated on the element type: Vector(Float32) or Vector(Int8) widened to f32;
 //  (2) the batched query x corpus similarity GEMM on the Hopper tensor cores:
 //      TMA (cp.async.bulk.tensor, multicast across a cluster) -> 128B-swizzled shared memory ->
-//      wgmma (bf16 in, f32 accumulators in registers) -> epilogue on the accumulator fragment that
-//      turns dot products into similarities and keeps only entries that beat the per-query
-//      boundary (the k'-th best so far), i.e. the score matrix is never written to HBM.
+//      wgmma (bf16 in, f32 accumulators, for Float32 corpora; s8 in, exact s32 accumulators, for
+//      Int8 corpora) -> epilogue on the accumulator fragment that turns dot products into
+//      similarities and keeps only entries that beat the per-query boundary (the k'-th best so
+//      far), i.e. the score matrix is never written to HBM.
 #pragma once
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -67,10 +71,11 @@ __device__ __forceinline__ float exact_cosine(const float* __restrict__ a, const
   return __fsub_rn(1.0f, __fdiv_rn(ab, __fmul_rn(__fsqrt_rn(aa), __fsqrt_rn(bb))));
 }
 // l2_distance: strictly sequential f32 fold of (a-b)^2, then sqrt
-__device__ __forceinline__ float exact_l2(const float* __restrict__ a, const float* __restrict__ b, int dim) {
+template <typename T>
+__device__ __forceinline__ float exact_l2(const T* __restrict__ a, const T* __restrict__ b, int dim) {
   float acc = 0.0f;
   for (int i = 0; i < dim; ++i) {
-    float d = __fsub_rn(a[i], b[i]);
+    float d = __fsub_rn((float)a[i], (float)b[i]);
     acc = __fadd_rn(acc, __fmul_rn(d, d));
   }
   return __fsqrt_rn(acc);
@@ -79,12 +84,22 @@ __device__ __forceinline__ float exact_distance(int kind, const float* a, const 
   return kind == DBX_DIST_COSINE ? exact_cosine(a, b, dim) : exact_l2(a, b, dim);
 }
 
+// Vector(Int8) arguments (calculate_distance, scalars/vector.rs:515-524) are widened element by
+// element (`*v as f32`) and then go through the same f32 functions.  The widening is exact (every
+// value is an integer in [-128, 127]), so the int8 instantiations below compute literally the
+// reference's f32 expression over the widened values, bit for bit, at every dim.  For int8 the
+// f32 arithmetic is even exact in most cases: every product has magnitude <= 2^14 and every
+// (a-b)^2 <= 65 025, so the sums stay exact while every partial sum is <= 2^24 — for cosine
+// (the 8-way fold) for every input with dim <= 1024, for L2 (a sequential fold of non-negative
+// terms) for every input with dim <= 258 and, beyond, for every pair with sum S <= 2^24 (once
+// S > 2^24 the fold's result is >= 2^24).
+
 // Coalesced form of exact_cosine: the 8 lanes of a group own the 8 interleaved accumulators of
 // ONE row (lane j accumulates elements 8c+j, c ascending — the same chains in the same order),
 // so a group reads one 32-byte sector per step; the fold and the tail are then done redundantly
 // by every lane of the group.  All 32 lanes of the warp must call this together.
-__device__ __forceinline__ float exact_cosine_g8(const float* __restrict__ a, const float* __restrict__ b, int dim,
-                                                 int lane) {
+template <typename T>
+__device__ __forceinline__ float exact_cosine_g8(const T* __restrict__ a, const T* __restrict__ b, int dim, int lane) {
   const int sub = lane & 7, gbase = lane & 24;
   float aa = 0.0f, bb = 0.0f, ab = 0.0f;
   const int n_chunks = dim >> 3;
@@ -92,7 +107,7 @@ __device__ __forceinline__ float exact_cosine_g8(const float* __restrict__ a, co
   for (; c + 8 <= n_chunks; c += 8) {
     float x[8], y[8];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) { x[u] = __ldg(a + (c + u) * 8 + sub); y[u] = __ldg(b + (c + u) * 8 + sub); }
+    for (int u = 0; u < 8; ++u) { x[u] = (float)__ldg(a + (c + u) * 8 + sub); y[u] = (float)__ldg(b + (c + u) * 8 + sub); }
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       aa = __fadd_rn(aa, __fmul_rn(x[u], x[u]));
@@ -101,7 +116,7 @@ __device__ __forceinline__ float exact_cosine_g8(const float* __restrict__ a, co
     }
   }
   for (; c < n_chunks; ++c) {
-    const float x = __ldg(a + c * 8 + sub), y = __ldg(b + c * 8 + sub);
+    const float x = (float)__ldg(a + c * 8 + sub), y = (float)__ldg(b + c * 8 + sub);
     aa = __fadd_rn(aa, __fmul_rn(x, x));
     bb = __fadd_rn(bb, __fmul_rn(y, y));
     ab = __fadd_rn(ab, __fmul_rn(x, y));
@@ -115,7 +130,7 @@ __device__ __forceinline__ float exact_cosine_g8(const float* __restrict__ a, co
   }
   float saa = fold8(paa), sbb = fold8(pbb), sab = fold8(pab);
   for (int i = n_chunks * 8; i < dim; ++i) {
-    const float x = __ldg(a + i), y = __ldg(b + i);
+    const float x = (float)__ldg(a + i), y = (float)__ldg(b + i);
     saa = __fadd_rn(saa, __fmul_rn(x, x));
     sbb = __fadd_rn(sbb, __fmul_rn(y, y));
     sab = __fadd_rn(sab, __fmul_rn(x, y));
@@ -123,9 +138,10 @@ __device__ __forceinline__ float exact_cosine_g8(const float* __restrict__ a, co
   return __fsub_rn(1.0f, __fdiv_rn(sab, __fmul_rn(__fsqrt_rn(saa), __fsqrt_rn(sbb))));
 }
 
-// calculate_distance (scalars/vector.rs:497-556), either side may be const.
+// calculate_distance (scalars/vector.rs:497-556), either side may be const; T = float or int8_t.
 // cosine: 8 lanes per row (coalesced sectors); L2 (one strictly sequential chain): one thread per row.
-__global__ void distance_rows_kernel(int kind, const float* lhs, int lhs_const, const float* rhs, int rhs_const,
+template <typename T>
+__global__ void distance_rows_kernel(int kind, const T* lhs, int lhs_const, const T* rhs, int rhs_const,
                                      int64_t rows, int dim, const uint8_t* lv, int64_t lv_off, const uint8_t* rv,
                                      int64_t rv_off, float* out, uint8_t* out_valid_bytes) {
   if (kind == DBX_DIST_COSINE) {
@@ -147,8 +163,8 @@ __global__ void distance_rows_kernel(int kind, const float* lhs, int lhs_const, 
   }
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x) {
     bool ok = (!lv || bit_test(lv, lv_off + r)) && (!rv || bit_test(rv, rv_off + r));
-    const float* a = lhs + (lhs_const ? 0 : r * dim);
-    const float* b = rhs + (rhs_const ? 0 : r * dim);
+    const T* a = lhs + (lhs_const ? 0 : r * dim);
+    const T* b = rhs + (rhs_const ? 0 : r * dim);
     out[r] = ok ? exact_l2(a, b, dim) : 0.0f;
     if (out_valid_bytes) out_valid_bytes[r] = ok ? 1 : 0;
   }
@@ -214,13 +230,56 @@ __global__ void prep_rows_kernel(const float* src, int64_t rows, int dim, int di
   if (unsafe_rows && lane == 0 && n_unsafe) atomicAdd(unsafe_rows, n_unsafe);
 }
 
+// i8 rows -> int8 operand of the similarity GEMM, zero-padded to dim_pad (a multiple of 128), plus
+//   sq[r]    = sum of x^2, exact in int32 (<= 2^14 dim < 2^31 for dim < 131 072);
+//   scale[r] = cosine: 1/|x| (f32 sqrt of the f32-rounded sum, then an f32 reciprocal; +inf for a
+//              zero row, whose similarities are then NaN and never pass the filter — harmless, its
+//              exact cosine distance is NaN for every query), L2: sum of x^2 rounded to f32 (the
+//              certificate's |q|^2; the GEMM's epilogue uses the exact sq).
+// max_norm_bits as for prep_rows_kernel.  int8 has no inf or NaN, so no row is outside the
+// certificate's range.
+__global__ void prep_rows_i8_kernel(const int8_t* src, int64_t rows, int dim, int dim_pad, int8_t* dst, int32_t* sq, float* scale,
+                                    int kind, unsigned int* max_norm_bits) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  float wmax = 0.0f;
+  for (int64_t r = warp; r < rows; r += n_warps) {
+    const int8_t* a = src + r * dim;
+    int8_t* d = dst + r * dim_pad;
+    int s = 0;
+    for (int i = lane * 4; i < dim_pad; i += 128) {
+      char4 v;
+      v.x = i < dim ? a[i] : 0;
+      v.y = i + 1 < dim ? a[i + 1] : 0;
+      v.z = i + 2 < dim ? a[i + 2] : 0;
+      v.w = i + 3 < dim ? a[i + 3] : 0;
+      s += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+      *reinterpret_cast<char4*>(d + i) = v;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float sf = __int2float_rn(s), nrm = __fsqrt_rn(sf);
+    if (lane == 0) {
+      sq[r] = s;
+      scale[r] = kind == DBX_DIST_COSINE ? __fdiv_rn(1.0f, nrm) : sf;
+    }
+    wmax = fmaxf(wmax, nrm);
+  }
+  if (max_norm_bits && lane == 0 && wmax > 0.0f) atomicMax(max_norm_bits, __float_as_uint(wmax));
+}
+
 // ---------------------------------------------------------------- wgmma GEMM with fused filter
 constexpr int kGemmBM = 128;      // queries per tile: two consumer warpgroups of 64 (wgmma M = 64)
 constexpr int kGemmBN = 128;      // corpus rows per tile  (wgmma N)
-constexpr int kGemmBK = 64;       // bf16 per k-block = 128 bytes = one swizzle row
+constexpr int kGemmBK = 64;       // bf16 per k-block = 128 bytes = one swizzle row (int8: 128 per k-block)
 constexpr int kGemmStages = 5;
 constexpr int kGemmThreads = 384; // warpgroup 0: TMA (one thread), warpgroups 1-2: wgmma + epilogue
-constexpr int kWgmmaK = 16;
+constexpr int kWgmmaK = 16;       // bf16 per wgmma k-step = 32 bytes (int8: 32 per k-step)
+constexpr int kKBlockBytes = 128;
+// elements of T per k-block: 64 bf16 or 128 int8, one 128-byte swizzle row either way
+template <typename T>
+constexpr int kBlockK = kKBlockBytes / (int)sizeof(T);
 constexpr uint32_t kStageBytesA = kGemmBM * kGemmBK * 2;
 constexpr uint32_t kStageBytesB = kGemmBN * kGemmBK * 2;
 constexpr int kCandStage = 512;   // staged survivors per consumer warp
@@ -243,13 +302,15 @@ struct KnnGemmParams {
   int32_t dim_pad;       // multiple of kGemmBK
   int64_t n0;            // first corpus row of this pass
   int64_t n_rows;        // corpus rows in this pass
-  const float* q_scale;  // L2: |q|^2                (cosine: unused, operands are pre-normalised)
-  const float* c_scale;  // L2: |c|^2 by global row  (cosine: unused)
+  const float* q_scale;  // bf16 L2: |q|^2; int8 cosine: 1/|q|   (bf16 cosine: unused, operands are pre-normalised)
+  const float* c_scale;  // bf16 L2: |c|^2; int8 cosine: 1/|c|, by global row
   const float* bound;    // per query: only score >= bound can still reach the top k'
   uint64_t* cand_key;    // (query << 32) | ~ordered(score): ascending sort = best first
   uint32_t* cand_row;    // corpus row
   unsigned long long* cand_count;
   int64_t cand_cap;
+  const int32_t* q_sq;   // int8 L2: exact |q|^2
+  const int32_t* c_sq;   // int8 L2: exact |c|^2 by global row
 };
 
 // arrive on the barrier at this offset in CTA `cta` of the cluster
@@ -326,6 +387,38 @@ __device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T, s8 in, s32 accumulators in registers, both K-major.
+// Integer wgmma has no negate / transpose immediates.  The accumulators are exact while |sum ab| <
+// 2^31, i.e. for dim < 131 072 (every product is <= 2^14 in magnitude).
+__device__ __forceinline__ void wgmma_m64n128k32_s8(int32_t (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// Similarity of an int8 pair from the exact integer dot product ab (larger = closer):
+//   cosine: ab / (|q| |c|) = (f32(ab) * (1/|q|)) * (1/|c|), a few f32 roundings of a value in [-1, 1];
+//   L2:     -S with S = |q|^2 + |c|^2 - 2ab computed exactly in 64-bit integers, rounded once to f32.
+__device__ __forceinline__ float i8_score(bool is_l2, int32_t ab, float q_inv, float c_inv, int32_t q_sq, int32_t c_sq) {
+  if (is_l2) return __ll2float_rn(2LL * ab - (long long)q_sq - (long long)c_sq);
+  return __fmul_rn(__fmul_rn(__int2float_rn(ab), q_inv), c_inv);
+}
 __device__ __forceinline__ uint32_t f32_to_ordered32(float f) {
   if (f != f) return 0u;  // NaN: worst similarity
   uint32_t b = __float_as_uint(f);
@@ -355,7 +448,11 @@ __device__ __forceinline__ void flush_stage(const uint64_t* skey, const uint32_t
 // the query blocks first, so a corpus tile is fetched from HBM once and re-read from L2.
 // Each consumer warpgroup multiplies 64 of the tile's 128 queries with wgmma and filters its
 // accumulator fragment in registers, so the score matrix is never written anywhere.
-template <int C>
+// T = __nv_bfloat16 (Float32 corpora) or int8_t (Int8 corpora): a k-block is one 128-byte swizzle
+// row of either, split into four 32-byte wgmma k-steps, so the producer, the barriers, the stages,
+// the multicast and the candidate staging are the same bytes for both; only the MMA instruction,
+// the accumulator type and the score differ.
+template <int C, typename T>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                        const __grid_constant__ KnnGemmParams p) {
@@ -367,7 +464,9 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
   const int n_mgrp = p.nq_pad / (kGemmBM * C);  // groups of C query blocks
   const int64_t n_nblk = (p.n_rows + kGemmBN - 1) / kGemmBN;
   const int64_t n_tiles = n_nblk * n_mgrp;      // cluster-level tiles
-  const int n_kblk = p.dim_pad / kGemmBK;
+  constexpr bool kI8 = std::is_same<T, int8_t>::value;
+  constexpr int kBK = kBlockK<T>;
+  const int n_kblk = p.dim_pad / kBK;
   constexpr uint16_t kMask = (uint16_t)((1u << C) - 1u);
   constexpr int kSliceRows = kGemmBN / C;       // corpus rows this CTA fetches for the whole cluster
 
@@ -392,11 +491,11 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         for (int kb = 0; kb < n_kblk; ++kb) {
           mbar_wait(&sm.empty_bar[stage], phase ^ 1);  // all C CTAs have consumed this slot
           mbar_expect_tx(&sm.full_bar[stage], kStageBytesA + kStageBytesB);
-          tma_load_2d(&tmap_q, &sm.full_bar[stage], sm.a[stage], kb * kGemmBK, m_blk * kGemmBM);
+          tma_load_2d(&tmap_q, &sm.full_bar[stage], sm.a[stage], kb * kBK, m_blk * kGemmBM);
           if (C > 1)
-            tma_load_2d_multicast(&tmap_c, &sm.full_bar[stage], sm.b[stage] + cta_rank * (kSliceRows * kGemmBK * 2), kb * kGemmBK, row_b, kMask);
+            tma_load_2d_multicast(&tmap_c, &sm.full_bar[stage], sm.b[stage] + cta_rank * (kSliceRows * kKBlockBytes), kb * kBK, row_b, kMask);
           else
-            tma_load_2d(&tmap_c, &sm.full_bar[stage], sm.b[stage], kb * kGemmBK, row_b);
+            tma_load_2d(&tmap_c, &sm.full_bar[stage], sm.b[stage], kb * kBK, row_b);
           if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -413,15 +512,15 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     const int wg = cw >> 2;             // queries [64*wg, +64) of the tile
     const uint32_t tid_wg = threadIdx.x & 127;
     const bool is_l2 = p.kind != DBX_DIST_COSINE;
-    // accumulator fragment of m64nNk16: register 4j + 2h + e holds row 16*(warp%4) + lane/4 + 8h,
-    // column 8j + 2*(lane%4) + e
+    // accumulator fragment of m64nNk16 (and m64nNk32): register 4j + 2h + e holds row
+    // 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + e
     const int col_l = 2 * (lane & 3);
     int stage = 0;
     uint32_t phase = 0;
     int stage_cnt = 0;  // warp-uniform
-    float acc[64];
+    typename std::conditional<kI8, int32_t, float>::type acc[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+    for (int i = 0; i < 64; ++i) acc[i] = 0;
     auto release = [&](int s) {  // one arrival per consumer warpgroup on slot s of every CTA in the cluster
       if (tid_wg < (uint32_t)C) {
         if (C > 1) mbar_arrive_cluster(&sm.empty_bar[s], tid_wg); else mbar_arrive(&sm.empty_bar[s]);
@@ -434,10 +533,14 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
       for (int kb = 0; kb < n_kblk; ++kb) {
         mbar_wait(&sm.full_bar[stage], phase);
         wgmma_fence();
-        const uint32_t a_addr = smem_u32(sm.a[stage]) + (uint32_t)wg * (64 * kGemmBK * 2), b_addr = smem_u32(sm.b[stage]);
+        const uint32_t a_addr = smem_u32(sm.a[stage]) + (uint32_t)wg * (64 * kKBlockBytes), b_addr = smem_u32(sm.b[stage]);
 #pragma unroll
-        for (int k = 0; k < kGemmBK / kWgmmaK; ++k)
-          wgmma_m64n128k16_bf16(acc, make_smem_desc(a_addr + k * kWgmmaK * 2), make_smem_desc(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+        for (int k = 0; k < kGemmBK / kWgmmaK; ++k) {  // four 32-byte k-steps
+          if constexpr (kI8)
+            wgmma_m64n128k32_s8(acc, make_smem_desc(a_addr + k * 32), make_smem_desc(b_addr + k * 32), (kb | k) != 0 ? 1u : 0u);
+          else
+            wgmma_m64n128k16_bf16(acc, make_smem_desc(a_addr + k * kWgmmaK * 2), make_smem_desc(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+        }
         wgmma_commit();
         if (prev >= 0) { wgmma_wait<1>(); release(prev); }  // the previous k-block's MMAs are done with their slot
         prev = stage;
@@ -449,11 +552,17 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
       const int q_a = m_blk * kGemmBM + wg * 64 + (cw & 3) * 16 + (lane >> 2);
       int qs[2];
       float qq[2], bnd[2];
+      int32_t qsq[2] = {0, 0};  // int8 L2
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         qs[h] = q_a + 8 * h;
         const bool q_ok = qs[h] < p.nq;
-        qq[h] = (q_ok && is_l2) ? p.q_scale[qs[h]] : 0.0f;
+        if constexpr (kI8) {
+          qq[h] = (q_ok && !is_l2) ? p.q_scale[qs[h]] : 0.0f;
+          qsq[h] = (q_ok && is_l2) ? p.q_sq[qs[h]] : 0;
+        } else {
+          qq[h] = (q_ok && is_l2) ? p.q_scale[qs[h]] : 0.0f;
+        }
         bnd[h] = q_ok ? p.bound[qs[h]] : __int_as_float(0x7f800000);  // +inf: nothing passes
       }
       const int64_t row0 = p.n0 + n_blk * kGemmBN;
@@ -466,7 +575,16 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         for (int jj = 0; jj < 4; ++jj) {
           const int col = (c * 4 + jj) * 8 + col_l;
           float cc[2] = {0.0f, 0.0f};
-          if (is_l2) {
+          int32_t csq[2] = {0, 0};  // int8 L2
+          if constexpr (kI8) {
+            if (is_l2) {
+              if (col < left) csq[0] = __ldg(p.c_sq + row0 + col);
+              if (col + 1 < left) csq[1] = __ldg(p.c_sq + row0 + col + 1);
+            } else {
+              if (col < left) cc[0] = __ldg(p.c_scale + row0 + col);
+              if (col + 1 < left) cc[1] = __ldg(p.c_scale + row0 + col + 1);
+            }
+          } else if (is_l2) {
             if (col < left) cc[0] = __ldg(p.c_scale + row0 + col);
             if (col + 1 < left) cc[1] = __ldg(p.c_scale + row0 + col + 1);
           }
@@ -475,10 +593,15 @@ knn_gemm_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int idx = jj * 4 + h * 2 + e;
-              float s = acc[(c * 4 + jj) * 4 + h * 2 + e];
-              // cosine: operands are pre-normalised, the accumulator IS the similarity;
-              // L2: score = -(|q|^2 + |c|^2 - 2 q.c)   (larger = closer)
-              if (is_l2) s = 2.0f * s - qq[h] - cc[e];
+              float s;
+              if constexpr (kI8) {
+                s = i8_score(is_l2, acc[(c * 4 + jj) * 4 + h * 2 + e], qq[h], cc[e], qsq[h], csq[e]);
+              } else {
+                s = acc[(c * 4 + jj) * 4 + h * 2 + e];
+                // cosine: operands are pre-normalised, the accumulator IS the similarity;
+                // L2: score = -(|q|^2 + |c|^2 - 2 q.c)   (larger = closer)
+                if (is_l2) s = 2.0f * s - qq[h] - cc[e];
+              }
               sc[idx] = s;
               pass |= (s >= bnd[h] && col + e < left) ? (1u << idx) : 0u;
             }
@@ -548,6 +671,29 @@ __global__ void knn_ref_filter_kernel(const __nv_bfloat16* q, const __nv_bfloat1
     float dot = 0.0f;
     for (int k = 0; k < p.dim_pad; ++k) dot += __bfloat162float(a[k]) * __bfloat162float(b[k]);
     const float s = p.kind == DBX_DIST_COSINE ? dot : 2.0f * dot - p.q_scale[qi] - p.c_scale[r];
+    if (s >= p.bound[qi]) {
+      unsigned long long pos = atomicAdd(p.cand_count, 1ULL);
+      if ((int64_t)pos < p.cand_cap) {
+        p.cand_key[pos] = ((uint64_t)(uint32_t)qi << 32) | (uint64_t)(~f32_to_ordered32(s));
+        p.cand_row[pos] = (uint32_t)r;
+      }
+    }
+  }
+}
+
+// Reference similarity pass for int8 operands on CUDA cores: exact int32 dot product over the same
+// padded operands, the same score and the same filter as the int8 wgmma kernel (DBX_KNN_REF_GEMM=1).
+__global__ void knn_ref_filter_i8_kernel(const int8_t* q, const int8_t* c, const __grid_constant__ KnnGemmParams p) {
+  const int64_t total = (int64_t)p.nq * p.n_rows;
+  const bool is_l2 = p.kind != DBX_DIST_COSINE;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int qi = (int)(i / p.n_rows);
+    const int64_t r = p.n0 + i % p.n_rows;
+    const int8_t* a = q + (int64_t)qi * p.dim_pad;
+    const int8_t* b = c + r * p.dim_pad;
+    int32_t dot = 0;
+    for (int k = 0; k < p.dim_pad; ++k) dot += (int32_t)a[k] * (int32_t)b[k];
+    const float s = is_l2 ? i8_score(true, dot, 0.0f, 0.0f, p.q_sq[qi], p.c_sq[r]) : i8_score(false, dot, p.q_scale[qi], p.c_scale[r], 0, 0);
     if (s >= p.bound[qi]) {
       unsigned long long pos = atomicAdd(p.cand_count, 1ULL);
       if ((int64_t)pos < p.cand_cap) {

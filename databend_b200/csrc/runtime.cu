@@ -296,7 +296,7 @@ int32_t pull_owned_block(std::unique_ptr<OwnedBlock>& result_dev, int device, cu
     c.mem = DBX_MEM_HOST;
     if (dc.is_const) { hb->cols.push_back(c); continue; }
     size_t bytes = dc.dtype == DBX_BOOL ? (size_t)(dc.data_bit_offset + dc.len + 7) / 8
-                 : dc.dtype == DBX_VEC_F32 ? (size_t)dc.len * 4 * dc.vec_dim : (size_t)dc.len * dtype_size(dc.dtype);
+                 : (size_t)dc.len * column_row_bytes(dc.dtype, dc.vec_dim);
     void* hp = nullptr;
     DBX_CUDA_TRY(err, pinned_alloc(bytes, &hp));
     hb->host_allocs.push_back(hp);

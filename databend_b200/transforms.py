@@ -102,11 +102,11 @@ def _block_from_c(b: abi.Block, device: int) -> DataBlock:
             if nb:
                 C.memmove(arr.ctypes.data, c.data, nb)
             col = Column(abi.BOOL, n, data=arr, data_bit_offset=c.data_bit_offset)
-        elif c.dtype == abi.VEC_F32:
-            arr = np.empty((n, c.vec_dim), dtype=np.float32)
+        elif c.dtype in (abi.VEC_F32, abi.VEC_I8):
+            arr = np.empty((n, c.vec_dim), dtype=np.float32 if c.dtype == abi.VEC_F32 else np.int8)
             if n:
                 C.memmove(arr.ctypes.data, c.data, arr.nbytes)
-            col = Column(abi.VEC_F32, n, data=arr, vec_dim=c.vec_dim)
+            col = Column(c.dtype, n, data=arr, vec_dim=c.vec_dim)
         else:
             nd = np_dtype(c.dtype)
             arr = np.empty(n, dtype=nd)

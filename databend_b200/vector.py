@@ -32,7 +32,9 @@ def _kind(name_or_kind) -> int:
 
 def eval_distance(fn: str, lhs: Column, rhs: Column, device: int = 0) -> Column:
     """ScalarFunction::eval for `cosine_distance(lhs, rhs)` / `l2_distance(lhs, rhs)`.
-    Either side may be a const column (one vector); NULL on either side gives NULL.
+    Either side may be a const column (one vector); NULL on either side gives NULL.  Vector(Int8)
+    sides are widened to f32 as in the reference; a Vector(Int8) / Vector(Float32) pair gives 0.0 on
+    every row (NULL when the result is Nullable).
     Returns a Float32 column (Nullable when an input is)."""
     kind = _kind(fn)
     rows = rhs.length if lhs.is_const else lhs.length
@@ -54,26 +56,35 @@ def eval_distance(fn: str, lhs: Column, rhs: Column, device: int = 0) -> Column:
 
 
 def _vector_as_c(col: Column):
-    """dbx_column of a Vector(Float32) entry; a const side carries its single vector in `data`."""
+    """dbx_column of a Vector(Float32) / Vector(Int8) entry; a const side carries its single vector in
+    `data`, in the column's element type."""
     if col.is_const:
         c = abi.Column()
-        c.dtype, c.is_const, c.len, c.mem = abi.VEC_F32, 1, col.length, abi.MEM_HOST
+        c.dtype, c.is_const, c.len, c.mem = col.dtype, 1, col.length, abi.MEM_HOST
         keep = None
         if col.const_value is None:
             c.konst.is_null = 1
             c.vec_dim = col.vec_dim
         else:
-            keep = np.ascontiguousarray(col.const_value, dtype=np.float32)
+            keep = np.ascontiguousarray(col.const_value, dtype=np.int8 if col.dtype == abi.VEC_I8 else np.float32)
             c.vec_dim = keep.shape[-1]
             c.data = keep.ctypes.data
         return c, keep
     return col.as_c(), None
 
 
-def const_vector(value, n: int, dim: Optional[int] = None) -> Column:
-    """BlockEntry::Const(Scalar::Vector(..), DataType::Vector, n)."""
-    v = None if value is None else np.ascontiguousarray(value, dtype=np.float32)
-    return Column(abi.VEC_F32, n, is_const=True, const_value=v, vec_dim=(dim if v is None else v.shape[-1]))
+def const_vector(value, n: int, dim: Optional[int] = None, dtype: Optional[int] = None) -> Column:
+    """BlockEntry::Const(Scalar::Vector(..), DataType::Vector, n).  An int8 array gives a Vector(Int8)
+    constant (kept int8), anything else a Vector(Float32) one; `dtype` (abi.VEC_F32 / abi.VEC_I8)
+    picks the type of a NULL constant."""
+    if value is None:
+        return Column(abi.VEC_F32 if dtype is None else dtype, n, is_const=True, const_value=None, vec_dim=dim)
+    if dtype is None:
+        dtype = abi.VEC_I8 if np.asarray(value).dtype == np.int8 else abi.VEC_F32
+    if dtype == abi.VEC_I8 and np.asarray(value).dtype != np.int8:
+        raise TypeError("const_vector: a Vector(Int8) constant takes int8 values")
+    v = np.ascontiguousarray(value, dtype=np.int8 if dtype == abi.VEC_I8 else np.float32)
+    return Column(dtype, n, is_const=True, const_value=v, vec_dim=v.shape[-1])
 
 
 class VectorTopN:

@@ -62,7 +62,7 @@ typedef enum dbx_status {
 } dbx_status;
 
 /* ------------------------------------------------------------- data types */
-/* NumberDataType subset (src/query/expression/src/types/number.rs) + Boolean + Vector(Float32) */
+/* NumberDataType subset (src/query/expression/src/types/number.rs) + Boolean + Vector(Float32 | Int8) */
 typedef enum dbx_dtype {
   DBX_BOOL = 0, /* bit-packed, LSB first (Bitmap) */
   DBX_I8 = 1,
@@ -75,7 +75,9 @@ typedef enum dbx_dtype {
   DBX_U64 = 8,
   DBX_F32 = 9,
   DBX_F64 = 10,
-  DBX_VEC_F32 = 11 /* VectorColumn::Float32((Buffer<F32>, dim)), flat row-major (types/vector.rs:377-380) */
+  DBX_VEC_F32 = 11, /* VectorColumn::Float32((Buffer<F32>, dim)), flat row-major (types/vector.rs:377-380) */
+  DBX_VEC_I8 = 12   /* VectorColumn::Int8((Buffer<i8>, dim)), flat row-major i8[len * vec_dim]; carried by the
+                     * block kernels, dbx_eval_distance and dbx_knn_*; every other operator refuses it */
 } dbx_dtype;
 
 /* OR-ed into the entries of dbx_op_create's input_types[] when the column's DataType is
@@ -102,9 +104,9 @@ typedef struct dbx_column {
   int32_t dtype;               /* dbx_dtype */
   int32_t mem;                 /* dbx_mem: where data/validity live */
   int32_t is_const;
-  int32_t vec_dim;             /* DBX_VEC_F32 only */
+  int32_t vec_dim;             /* DBX_VEC_F32 / DBX_VEC_I8 only */
   int64_t len;                 /* rows */
-  const void* data;            /* T[len] (bool: bit-packed; vec: f32[len*vec_dim]) */
+  const void* data;            /* T[len] (bool: bit-packed; vec: f32 / i8 [len*vec_dim]) */
   int64_t data_bit_offset;     /* DBX_BOOL only: bit offset of row 0 */
   const uint8_t* validity;     /* NULL = no nulls; else LSB-first bitmap, 1 = valid */
   int64_t validity_bit_offset;
@@ -615,14 +617,20 @@ int32_t dbx_eval_scalar(int32_t device, const dbx_expr* expr, const dbx_block* b
                         int32_t* out_dtype, int64_t* first_error_row);
 
 /* ScalarFunction::eval replacement for the vector distances (scalars/vector.rs:497-556):
- * out[i] = distance(lhs[i], rhs[i]) row-wise, either side may be const.  f32 result. */
+ * out[i] = distance(lhs[i], rhs[i]) row-wise, either side may be const.  f32 result.
+ * Arguments: DBX_VEC_F32 or DBX_VEC_I8.  Int8 values are widened to f32 and go through the f32
+ * functions, as in the reference (bit-identical; a zero vector gives NaN for cosine).  A mixed
+ * Int8 / Float32 pair is not an error and its dims are not compared: every row is 0.0, or NULL
+ * when out->validity is given (the reference's invalid-row arm). */
 int32_t dbx_eval_distance(int32_t kind, int32_t device, const dbx_column* lhs, const dbx_column* rhs,
                           dbx_column* out /* caller-provided f32 buffer, mem as given */);
 
 /* Brute-force kNN: `ORDER BY cosine_distance(c, q) LIMIT k` for a batch of queries, i.e.
  * the EvalScalar -> TopN pipeline of SURVEY 3.5 fused: tensor-core GEMM for candidate
  * selection, exact fp32 re-evaluation of the returned distances.
- * corpus: DBX_VEC_F32 [n, dim]; queries: DBX_VEC_F32 [nq, dim];
+ * corpus: DBX_VEC_F32 or DBX_VEC_I8 [n, dim] (Int8: dim < 131072, int8 tensor cores with exact integer
+ * dot products); queries: the corpus's element type [nq, dim] (another element type is DBX_ERR_INVALID);
+ * no NULL vectors (DBX_ERR_UNSUPPORTED).
  * out_idx[nq*k] (int64 row ids), out_dist[nq*k] (f32), ascending by distance (NaN last). */
 typedef struct dbx_knn dbx_knn;
 int32_t dbx_knn_create(int32_t kind, int32_t device, const dbx_column* corpus, dbx_knn** out);

@@ -24,7 +24,7 @@ PRED_CMP, PRED_AND, PRED_OR, PRED_BOOLCOL, PRED_CONST = range(5)
 AGG_SUM, AGG_COUNT, AGG_AVG, AGG_MIN, AGG_MAX = range(5)
 
 # dbx_op_kind
-OP_FILTER, OP_AGG_PARTIAL, OP_AGG_FINAL, OP_TOPK, OP_JOIN = range(5)
+OP_FILTER, OP_AGG_PARTIAL, OP_AGG_FINAL, OP_TOPK, OP_JOIN, OP_WINDOW = range(6)
 
 DIST_COSINE, DIST_L2 = 0, 1
 JOIN_INNER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI, JOIN_LEFT = 0, 1, 2, 3
@@ -124,6 +124,52 @@ class TopkParams(C.Structure):
         ("extra_key_cols", C.c_int32 * (MAX_SORT_KEYS - 1)),
         ("extra_asc", C.c_int32 * (MAX_SORT_KEYS - 1)),
         ("extra_nulls_first", C.c_int32 * (MAX_SORT_KEYS - 1)),
+    ]
+
+
+# dbx_window_kind / dbx_frame_units / dbx_frame_bound
+(WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_PERCENT_RANK, WIN_CUME_DIST, WIN_NTILE, WIN_LAG, WIN_LEAD, WIN_NTH_VALUE,
+ WIN_AGGREGATE) = range(10)
+FRAME_ROWS, FRAME_RANGE = 0, 1
+BOUND_UNBOUNDED_PRECEDING, BOUND_PRECEDING, BOUND_CURRENT_ROW, BOUND_FOLLOWING, BOUND_UNBOUNDED_FOLLOWING = range(1, 6)
+MAX_WINDOW_FUNCS = 8
+
+
+class WindowFrame(C.Structure):
+    _fields_ = [
+        ("units", C.c_int32),
+        ("start", C.c_int32),
+        ("end", C.c_int32),
+        ("reserved", C.c_int32),
+        ("start_offset", C.c_int64),
+        ("end_offset", C.c_int64),
+    ]
+
+
+class WindowFunc(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32),
+        ("agg_kind", C.c_int32),
+        ("arg_col", C.c_int32),
+        ("default_col", C.c_int32),
+        ("n", C.c_int64),
+        ("ignore_nulls", C.c_int32),
+        ("distinct", C.c_int32),
+        ("frame", WindowFrame),
+    ]
+
+
+class WindowParams(C.Structure):
+    _fields_ = [
+        ("n_partition_cols", C.c_int32),
+        ("partition_cols", C.c_int32 * MAX_SORT_KEYS),
+        ("n_order_cols", C.c_int32),
+        ("order_cols", C.c_int32 * MAX_SORT_KEYS),
+        ("order_asc", C.c_int32 * MAX_SORT_KEYS),
+        ("order_nulls_first", C.c_int32 * MAX_SORT_KEYS),
+        ("n_funcs", C.c_int32),
+        ("reserved", C.c_int32),
+        ("funcs", WindowFunc * MAX_WINDOW_FUNCS),
     ]
 
 

@@ -332,6 +332,7 @@ Op* make_agg_final_op(const dbx_agg_params* p, const int32_t* types, int32_t n, 
 Op* make_filter_op(const dbx_predicate* p, const int32_t* types, int32_t n, const dbx_expr* comp, int32_t n_comp, int device, int32_t* st);
 Op* make_topk_op(const dbx_topk_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
 Op* make_join_op(const dbx_join_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
+Op* make_window_op(const dbx_window_params* p, const int32_t* types, int32_t n, int device, int32_t* st);
 
 }  // namespace dbx
 
@@ -417,7 +418,7 @@ int32_t dbx_op_create_computed(int32_t kind, const void* params, const int32_t* 
   if (n_computed < 0 || n_computed > DBX_MAX_COMPUTED_COLS) { g_create_error.set("dbx_op_create_computed: n_computed outside 0 .. DBX_MAX_COMPUTED_COLS"); return DBX_ERR_INVALID; }
   if (n_computed > 0 && !computed) { g_create_error.set("dbx_op_create_computed: null computed list"); return DBX_ERR_INVALID; }
   if (n_computed > 0 && n_input_cols + n_computed > 64) { g_create_error.set("dbx_op_create_computed: more than 64 input and computed columns"); return DBX_ERR_INVALID; }
-  if (n_computed > 0 && (kind == DBX_OP_TOPK || kind == DBX_OP_JOIN)) {
+  if (n_computed > 0 && (kind == DBX_OP_TOPK || kind == DBX_OP_JOIN || kind == DBX_OP_WINDOW)) {
     g_create_error.set("dbx_op_create_computed: computed columns are taken by the filter and aggregate operators only");
     return DBX_ERR_UNSUPPORTED;
   }
@@ -433,6 +434,7 @@ int32_t dbx_op_create_computed(int32_t kind, const void* params, const int32_t* 
     case DBX_OP_FILTER: op = make_filter_op((const dbx_predicate*)params, input_types, n_input_cols, computed, n_computed, device, &st); break;
     case DBX_OP_TOPK: op = make_topk_op((const dbx_topk_params*)params, input_types, n_input_cols, device, &st); break;
     case DBX_OP_JOIN: op = make_join_op((const dbx_join_params*)params, input_types, n_input_cols, device, &st); break;
+    case DBX_OP_WINDOW: op = make_window_op((const dbx_window_params*)params, input_types, n_input_cols, device, &st); break;
     default: g_create_error.set("dbx_op_create: unknown operator kind"); return DBX_ERR_INVALID;
   }
   if (!op) return st == DBX_OK ? DBX_ERR_INVALID : st;

@@ -26,63 +26,13 @@
 #include <algorithm>
 #include <vector>
 
-#include "radix_sort.cuh"
-#include "runtime.h"
+#include "sort_keys.cuh"
 
 namespace dbx {
 
 namespace {
 
-// ================================================================ key images
-// Key classes: VC_INT / VC_UINT / VC_FLT (Float64 bits) and KC_F32, a Float32 key carried in its own
-// 32 bits.  A float -> double -> float round trip quiets a signalling NaN on sm_90 (0x7F800001 comes
-// back as 0x7FC00001), and the result must return every row's key bit for bit.
-constexpr int KC_F32 = 3;
-inline int key_class(int dtype) {
-  if (dtype == DBX_F32) return KC_F32;
-  return dtype == DBX_U64 ? VC_UINT : (dtype_class(dtype) == VC_FLT ? VC_FLT : VC_INT);
-}
-
-__device__ __forceinline__ uint64_t key_to_ord(uint64_t bits, int cls, bool asc) {
-  uint64_t o;
-  if (cls == VC_FLT || cls == KC_F32) {
-    double d = cls == KC_F32 ? (double)__uint_as_float((uint32_t)bits) : __longlong_as_double((long long)bits);
-    if (d == 0.0) d = 0.0;  // -0 == +0
-    o = f64_to_ordered(d);
-  } else if (cls == VC_INT) {
-    o = bits ^ 0x8000000000000000ULL;
-  } else {
-    o = bits;
-  }
-  return asc ? o : ~o;
-}
-
-// integers sign- or zero-extended to 64 bits; Float32 keeps its own 32 bits (see KC_F32)
-__device__ __forceinline__ uint64_t load_widened(const DevCol& c, int64_t row, uint64_t pol) {
-  const char* base = (const char*)c.data;
-  switch (c.dtype) {
-    case DBX_I64: case DBX_U64: case DBX_F64: return ld_stream_u64(base + row * 8, pol);
-    case DBX_I32: return (uint64_t)(int64_t)(int32_t)ld_stream_u32(base + row * 4, pol);
-    case DBX_U32: case DBX_F32: return ld_stream_u32(base + row * 4, pol);
-    case DBX_I16: return (uint64_t)(int64_t)(int16_t)ld_stream_u16(base + row * 2, pol);
-    case DBX_U16: return ld_stream_u16(base + row * 2, pol);
-    case DBX_I8: return (uint64_t)(int64_t)(int8_t)ld_stream_u8(base + row, pol);
-    default: return ld_stream_u8(base + row, pol);
-  }
-}
-
-__device__ __forceinline__ void store_narrow_key(void* out, int64_t i, int dtype, uint64_t b) {
-  switch (dtype) {
-    case DBX_I8: case DBX_U8: ((uint8_t*)out)[i] = (uint8_t)b; break;
-    case DBX_I16: case DBX_U16: ((uint16_t*)out)[i] = (uint16_t)b; break;
-    case DBX_I32: case DBX_U32: case DBX_F32: ((uint32_t*)out)[i] = (uint32_t)b; break;
-    default: ((uint64_t*)out)[i] = b; break;
-  }
-}
-
-inline int grid_1d(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)kNumSMs * 8)); }
-
-// (the radix sort lives in radix_sort.cuh)
+// (the key images and the multi-key sort live in sort_keys.cuh, the radix sort in radix_sort.cuh)
 // ================================================================ streaming top-k
 // Device state words of one candidate list
 enum : int { ST_COUNT = 0, ST_BOUND = 1, ST_OVERFLOW = 2, ST_WORDS = 4 };
@@ -429,56 +379,6 @@ __global__ void topk_emit_kernel(const __grid_constant__ EmitArgs a) {
       a.out_row[i] = (int64_t)a.rowid[j];
       a.out_valid_bytes[i] = 1;
     }
-  }
-}
-__global__ void pack_bits_kernel(const uint8_t* bytes, int64_t n, uint8_t* bits) {
-  const int64_t nb = (n + 7) / 8;
-  for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += (int64_t)gridDim.x * blockDim.x) {
-    uint32_t v = 0;
-    for (int k = 0; k < 8; ++k) {
-      const int64_t i = b * 8 + k;
-      if (i < n && bytes[i]) v |= 1u << k;
-    }
-    bits[b] = (uint8_t)v;
-  }
-}
-
-// ================================================================ full sort: ingest
-// Appends one chunk of the key column to the (ord, row id | NULL flag, original bits) arrays.
-__global__ void __launch_bounds__(256) sort_ingest_kernel(const __grid_constant__ DevCol col, int64_t n, int64_t row_base, int cls, int asc,
-                                                          uint64_t* ord, uint32_t* rid, uint64_t* bits, unsigned long long* n_null,
-                                                          unsigned long long* inexact) {
-  const uint64_t pol = make_policy_evict_first();
-  unsigned int nulls = 0;
-  bool lossy = false;  // -0.0 and NaN payloads do not survive key -> ordered image -> key
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const bool ok = !col.validity || bit_test(col.validity, col.vbit_off + i);
-    const uint64_t v = ok ? load_widened(col, i, pol) : 0;
-    ord[row_base + i] = ok ? key_to_ord(v, cls, asc != 0) : 0;  // NULL rows: placed by the extra pass on the flag
-    rid[row_base + i] = (uint32_t)(row_base + i) | (ok ? 0u : 0x80000000u);
-    if (bits) bits[row_base + i] = v;
-    nulls += !ok;
-    if (ok && cls == VC_FLT) {
-      const double d = __longlong_as_double((long long)v);
-      lossy |= (d != d && v != 0x7FF8000000000000ULL) || (d == 0.0 && (v >> 63));
-    } else if (ok && cls == KC_F32) {
-      const float f = __uint_as_float((uint32_t)v);
-      lossy |= (f != f && v != 0x7FC00000u) || (f == 0.0f && (v >> 31));
-    }
-  }
-  if (inexact && __any_sync(0xffffffffu, lossy) && (threadIdx.x & 31) == 0) *inexact = 1;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) nulls += __shfl_xor_sync(0xffffffffu, nulls, o);
-  if ((threadIdx.x & 31) == 0 && nulls) atomicAdd(n_null, (unsigned long long)nulls);
-}
-// Multi-column ORDER BY: the keys of column c in the order the less significant columns have
-// established so far (perm = sorted row id | flag of the previous step; nullptr = input order).
-__global__ void __launch_bounds__(256) sort_gather_kernel(const uint64_t* ord_c, const uint32_t* rid_c, const uint32_t* perm, int64_t n,
-                                                          uint64_t* o_ord, uint32_t* o_rid) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = perm ? (perm[i] & 0x7FFFFFFFu) : (uint32_t)i;
-    o_ord[i] = ord_c[r];
-    o_rid[i] = r | (rid_c[r] & 0x80000000u);
   }
 }
 struct SortEmitArgs {
@@ -1414,31 +1314,18 @@ class TopkOp : public Op {
     const uint64_t* sorted_ord = nullptr;
     const uint32_t* sorted_rid = nullptr;
     if (n_extra > 0 && n > 1) {
-      // least significant key first; every step is a STABLE sort of (key image, row id) in the order
-      // the previous steps established, so earlier keys dominate and input order breaks the last ties
       unsigned long long xn[DBX_MAX_SORT_KEYS] = {};
       DBX_CUDA_TRY(err, cudaMemcpyAsync(xn, x_cnt.p, 8 * (DBX_MAX_SORT_KEYS - 1), cudaMemcpyDeviceToHost, stream));
       DBX_CUDA_TRY(err, cudaStreamSynchronize(stream));
-      for (int i = 0; i < 2; ++i) { DBX_CUDA_TRY(err, w_ord[i].ensure((size_t)n * 8)); DBX_CUDA_TRY(err, w_rid[i].ensure((size_t)n * 4)); }
-      int res = 1;  // which work pair holds the current order (none yet: the first gather goes to pair 0)
-      const uint32_t* perm = nullptr;
-      for (int c = n_extra - 1; c >= -1; --c) {
-        const uint64_t* col_ord = c >= 0 ? (const uint64_t*)x_ord[c].p : (const uint64_t*)s_ord[0].p;
-        const uint32_t* col_rid = c >= 0 ? (const uint32_t*)x_rid[c].p : (const uint32_t*)s_rid[0].p;
-        const int64_t c_nulls = c >= 0 ? (int64_t)xn[c] : n_nulls;
-        const int c_nulls_first = c >= 0 ? prm.extra_nulls_first[c] : prm.nulls_first;
-        const int in = res ^ 1;
-        sort_gather_kernel<<<grid_1d(n), 256, 0, stream>>>(col_ord, col_rid, perm, n, (uint64_t*)w_ord[in].p, (uint32_t*)w_rid[in].p);
-        count_launch();
-        DBX_CUDA_TRY(err, cudaGetLastError());
-        int rb = 0;
-        DBX_TRY(sorter.sort(err, stream, (uint64_t*)w_ord[in].p, (uint64_t*)w_ord[in ^ 1].p, (uint32_t*)w_rid[in].p, (uint32_t*)w_rid[in ^ 1].p, n, 0,
-                            64, c_nulls > 0, c_nulls_first, c_nulls, &rb));
-        res = rb ? (in ^ 1) : in;
-        perm = (const uint32_t*)w_rid[res].p;
+      const uint64_t* k_ord[DBX_MAX_SORT_KEYS] = {(const uint64_t*)s_ord[0].p};
+      const uint32_t* k_rid[DBX_MAX_SORT_KEYS] = {(const uint32_t*)s_rid[0].p};
+      int64_t k_nulls[DBX_MAX_SORT_KEYS] = {n_nulls};
+      int32_t k_nulls_first[DBX_MAX_SORT_KEYS] = {prm.nulls_first};
+      for (int j = 0; j < n_extra; ++j) {
+        k_ord[1 + j] = (const uint64_t*)x_ord[j].p; k_rid[1 + j] = (const uint32_t*)x_rid[j].p;
+        k_nulls[1 + j] = (int64_t)xn[j]; k_nulls_first[1 + j] = prm.extra_nulls_first[j];
       }
-      sorted_ord = (const uint64_t*)w_ord[res].p;
-      sorted_rid = (const uint32_t*)w_rid[res].p;
+      DBX_TRY(sort_rows_by_keys(err, stream, sorter, 1 + n_extra, k_ord, k_rid, k_nulls, k_nulls_first, n, w_ord, w_rid, &sorted_ord, &sorted_rid));
     } else if (n > 1) {
       DBX_CUDA_TRY(err, s_ord[1].ensure((size_t)s_cap * 8));
       DBX_CUDA_TRY(err, s_rid[1].ensure((size_t)s_cap * 4));

@@ -376,6 +376,75 @@ class TransformTopN(_Op):
         return _block_from_c(b, self.device)
 
 
+_WIN_KINDS = {"row_number": abi.WIN_ROW_NUMBER, "rank": abi.WIN_RANK, "dense_rank": abi.WIN_DENSE_RANK,
+              "percent_rank": abi.WIN_PERCENT_RANK, "cume_dist": abi.WIN_CUME_DIST, "ntile": abi.WIN_NTILE, "lag": abi.WIN_LAG,
+              "lead": abi.WIN_LEAD, "nth_value": abi.WIN_NTH_VALUE, "last_value": abi.WIN_NTH_VALUE}
+_WIN_AGGS = {"sum": abi.AGG_SUM, "count": abi.AGG_COUNT, "avg": abi.AGG_AVG, "min": abi.AGG_MIN, "max": abi.AGG_MAX}
+_BOUNDS = {"unbounded_preceding": abi.BOUND_UNBOUNDED_PRECEDING, "preceding": abi.BOUND_PRECEDING, "current_row": abi.BOUND_CURRENT_ROW,
+           "following": abi.BOUND_FOLLOWING, "unbounded_following": abi.BOUND_UNBOUNDED_FOLLOWING}
+
+
+@dataclass
+class WindowFunc:
+    """One Window node: `name` is a ranking function, ntile, lag, lead, nth_value, last_value or an
+    aggregate (sum, count, avg, min, max; arg = -1 is count(*)).  `n`: ntile buckets, lag / lead offset,
+    nth_value index.  `default`: lag / lead default column (-1: NULL).  `frame` (aggregates and
+    nth_value only): (units "rows" | "range", start, end), a bound being "unbounded_preceding",
+    ("preceding", k), "current_row", ("following", k) or "unbounded_following"."""
+    name: str
+    arg: int = -1
+    n: int = 0
+    default: int = -1
+    frame: Optional[Tuple] = None
+    ignore_nulls: bool = False
+    distinct: bool = False
+
+    def to_c(self, out: abi.WindowFunc):
+        if self.name in _WIN_AGGS:
+            out.kind, out.agg_kind = abi.WIN_AGGREGATE, _WIN_AGGS[self.name]
+        else:
+            out.kind = _WIN_KINDS[self.name]
+        out.arg_col, out.default_col, out.n = self.arg, self.default, self.n
+        out.ignore_nulls, out.distinct = int(self.ignore_nulls), int(self.distinct)
+        if self.frame is not None:
+            units, start, end = self.frame
+            out.frame.units = abi.FRAME_RANGE if units == "range" else abi.FRAME_ROWS
+            for b, kind_f, off_f in ((start, "start", "start_offset"), (end, "end", "end_offset")):
+                name, off = (b, 0) if isinstance(b, str) else b
+                setattr(out.frame, kind_f, _BOUNDS[name])
+                setattr(out.frame, off_f, off)
+
+
+class TransformWindow(_Op):
+    """WindowPartition + its chain of Window nodes (physical_window{,_partition}.rs, TransformWindow
+    transform_window.rs) as one DBX_OP_WINDOW.  `transform(block)` buffers the block on the device;
+    `on_finish()` returns one block: every input column in window order (grouped by partition, sorted
+    by the order keys inside it, ties in input order), then one column per function."""
+
+    def __init__(self, partition_by: Sequence[int], order_by: Sequence[Tuple[int, bool, bool]], funcs: Sequence[WindowFunc],
+                 input_types: Sequence[int], device: int = 0):
+        """order_by: (offset, asc, nulls_first) per ORDER BY key."""
+        p = abi.WindowParams()
+        p.n_partition_cols, p.n_order_cols, p.n_funcs = len(partition_by), len(order_by), len(funcs)
+        for i, c in enumerate(partition_by[:abi.MAX_SORT_KEYS]):
+            p.partition_cols[i] = c
+        for i, (c, a, nf) in enumerate(order_by[:abi.MAX_SORT_KEYS]):
+            p.order_cols[i], p.order_asc[i], p.order_nulls_first[i] = c, int(a), int(nf)
+        for i, f in enumerate(funcs[:abi.MAX_WINDOW_FUNCS]):
+            f.to_c(p.funcs[i])
+        super().__init__(abi.OP_WINDOW, p, input_types, device)
+
+    def transform(self, block: DataBlock) -> List[DataBlock]:
+        self.push(block)
+        return []
+
+    def on_finish(self, out_mem: int = abi.MEM_HOST):
+        """The result as a host DataBlock, or (out_mem = MEM_DEVICE) the library-owned abi.Block."""
+        self.finish()
+        b = self.pull_c(out_mem)
+        return _block_from_c(b, self.device) if out_mem == abi.MEM_HOST else b
+
+
 def _key_list(key) -> List[int]:
     return [int(key)] if isinstance(key, (int, np.integer)) else [int(k) for k in key]
 

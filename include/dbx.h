@@ -212,6 +212,93 @@ typedef struct dbx_topk_params {
   int32_t extra_nulls_first[DBX_MAX_SORT_KEYS - 1];
 } dbx_topk_params;
 
+/* ---------------------------------------------------------------- window */
+/* One WindowPartition (physical_window_partition.rs) and the chain of Window nodes that share its
+ * PARTITION BY / ORDER BY (physical_window.rs), run as one DBX_OP_WINDOW: the input is sorted once
+ * by (partition keys, order keys) and every function appends one result column.
+ *   Keys: at most DBX_MAX_SORT_KEYS partition and order keys together, any numeric type, nullable or
+ *     not (more keys: DBX_ERR_INVALID).  Keys compare as the reference's ScalarRef equality does in
+ *     advance_partition / are_peers: floats as OrderedFloat (NaN == NaN, -0 == +0), NULL equals NULL
+ *     and differs from every value.  n_partition_cols = 0 is one partition.
+ *   Result: ONE library-owned block: every input column permuted into window order (numeric, Boolean,
+ *     Vector, Nullable and Const columns as the block kernels carry them), then one column per function
+ *     in list order.  Rows come grouped by partition, sorted inside each partition by the order keys;
+ *     ties on the order keys keep input order (the reference leaves their order unspecified).  The order
+ *     of the partitions is unspecified.
+ *   Result types (WindowFunction::data_type): ROW_NUMBER, RANK, DENSE_RANK, NTILE: UInt64;
+ *     PERCENT_RANK, CUME_DIST: Float64; LAG / LEAD / NTH_VALUE: the argument type, Nullable unless a
+ *     default column is given and neither it nor the argument is nullable; AGGREGATE: the aggregate
+ *     path's types (sum: Int64 / UInt64 / Float64, avg: Float64, min / max: the argument type, all
+ *     Nullable; count: UInt64).
+ *   Frames: `frame` applies to AGGREGATE and NTH_VALUE and must be given for them; every other kind
+ *     gets the frame the binder gives it (type_check/window.rs:604-655) and must leave `frame` zeroed.
+ *     Frame results are those of TransformWindow::add_block's row loop (transform_window.rs:1003-1153):
+ *     bounds clamp at the partition's edges, a frame whose start bound lies after its end bound
+ *     (ROWS 1 FOLLOWING AND 1 PRECEDING) is empty on every row, and an empty frame gives NULL
+ *     (count: 0).  Sums and averages add the frame's rows in row order: integer ones exactly
+ *     (wrapping, as the aggregate path), Float ones bit-exactly when both frame bounds are offsets or
+ *     CURRENT ROW; a Float frame with an UNBOUNDED side is summed by a parallel scan, which rounds
+ *     differently from the reference's left-to-right sum (a relative error below n * 2^-52 of the sum
+ *     of magnitudes over the n rows of the partition).  min / max follow the aggregate path's rule for
+ *     floats: NaN is the greatest value and -0 orders below +0.
+ *   Cost: Float sums / averages and every min / max over a frame bounded on both sides (offsets or
+ *     CURRENT ROW, RANGE CURRENT ROW AND CURRENT ROW included) read each row's frame: O(rows x frame
+ *     width), where the width is at most start_offset + end_offset + 1 (ROWS) or the peer group (RANGE)
+ *     and never more than the partition.  Keeping the reference's row order is what makes those sums
+ *     bit-exact.  A plan with very wide two-sided frames over large partitions (ROWS BETWEEN 1000000
+ *     PRECEDING AND 1000000 FOLLOWING) is better written with an UNBOUNDED side, or kept on the CPU.
+ *     Every other function and frame costs O(rows) after the sort.
+ *   DBX_ERR_UNSUPPORTED: RANGE frames with an offset, IGNORE NULLS, DISTINCT window aggregates,
+ *     LAG / LEAD / NTH_VALUE of Boolean or Vector arguments (valid in the reference, not built here:
+ *     the argument gather carries numeric values only), more than 2^30 - 1 rows (a push that would
+ *     cross it is refused before anything is allocated for it).
+ *   DBX_ERR_INVALID: key, argument or default columns outside the schema, non-numeric keys, Vector or
+ *     Boolean aggregate arguments, a default column of another type than the argument, n_funcs outside
+ *     1 .. DBX_MAX_WINDOW_FUNCS, NTILE(0), negative frame offsets or NTH_VALUE index, a frame on a kind
+ *     that takes none. */
+#define DBX_MAX_WINDOW_FUNCS 8
+typedef enum dbx_window_kind {
+  DBX_WIN_ROW_NUMBER = 0, DBX_WIN_RANK = 1, DBX_WIN_DENSE_RANK = 2, DBX_WIN_PERCENT_RANK = 3, DBX_WIN_CUME_DIST = 4,
+  DBX_WIN_NTILE = 5,      /* n buckets (n >= 1) */
+  DBX_WIN_LAG = 6,        /* arg_col, n (offset; negative n is LEAD by -n, as the reference accepts), default_col (-1: NULL) */
+  DBX_WIN_LEAD = 7,
+  DBX_WIN_NTH_VALUE = 8,  /* arg_col, n >= 1 counting from the frame start; n = 0 is last_value */
+  DBX_WIN_AGGREGATE = 9   /* agg_kind (dbx_agg_kind), arg_col (-1: count(*)) */
+} dbx_window_kind;
+typedef enum dbx_frame_units { DBX_FRAME_ROWS = 0, DBX_FRAME_RANGE = 1 } dbx_frame_units;
+typedef enum dbx_frame_bound {  /* 0: no frame */
+  DBX_BOUND_UNBOUNDED_PRECEDING = 1, DBX_BOUND_PRECEDING = 2, DBX_BOUND_CURRENT_ROW = 3, DBX_BOUND_FOLLOWING = 4,
+  DBX_BOUND_UNBOUNDED_FOLLOWING = 5
+} dbx_frame_bound;
+typedef struct dbx_window_frame {  /* WindowFuncFrame */
+  int32_t units;        /* dbx_frame_units */
+  int32_t start, end;   /* dbx_frame_bound */
+  int32_t reserved;
+  int64_t start_offset; /* rows, for DBX_BOUND_PRECEDING / DBX_BOUND_FOLLOWING */
+  int64_t end_offset;
+} dbx_window_frame;
+typedef struct dbx_window_func {
+  int32_t kind;         /* dbx_window_kind */
+  int32_t agg_kind;     /* DBX_WIN_AGGREGATE: dbx_agg_kind */
+  int32_t arg_col;
+  int32_t default_col;  /* DBX_WIN_LAG / DBX_WIN_LEAD: -1 = NULL */
+  int64_t n;
+  int32_t ignore_nulls; /* IGNORE NULLS: DBX_ERR_UNSUPPORTED */
+  int32_t distinct;     /* DISTINCT aggregate: DBX_ERR_UNSUPPORTED */
+  dbx_window_frame frame;
+} dbx_window_func;
+typedef struct dbx_window_params {
+  int32_t n_partition_cols;
+  int32_t partition_cols[DBX_MAX_SORT_KEYS];
+  int32_t n_order_cols;
+  int32_t order_cols[DBX_MAX_SORT_KEYS];
+  int32_t order_asc[DBX_MAX_SORT_KEYS];
+  int32_t order_nulls_first[DBX_MAX_SORT_KEYS];
+  int32_t n_funcs;
+  int32_t reserved;
+  dbx_window_func funcs[DBX_MAX_WINDOW_FUNCS];
+} dbx_window_params;
+
 /* ------------------------------------------------------------------ join */
 /* INNER: probe columns then build columns per matching pair (inner_join.rs:236-245).
  * LEFT_SEMI / LEFT_ANTI (probe side is "left"): the probe rows with at least one / with no match,
@@ -265,7 +352,8 @@ typedef enum dbx_op_kind {
   DBX_OP_AGG_PARTIAL = 1,         /* [TransformFilter ->] TransformPartialAggregate / PartialSingleStateAggregator */
   DBX_OP_AGG_FINAL = 2,           /* TransformFinalAggregate / FinalSingleStateAggregator */
   DBX_OP_TOPK = 3,                /* TransformSortPartial+merge with LIMIT / TransformPartialTopN+FinalTopN */
-  DBX_OP_JOIN = 4                 /* Join trait: add_block / final_build / probe_block / final_probe */
+  DBX_OP_JOIN = 4,                /* Join trait: add_block / final_build / probe_block / final_probe */
+  DBX_OP_WINDOW = 5               /* WindowPartition + its chain of Window nodes (TransformWindow) */
 } dbx_op_kind;
 
 typedef struct dbx_op dbx_op; /* opaque operator handle */
@@ -290,7 +378,8 @@ int32_t dbx_memcpy_d2d(int32_t device, void* dst, const void* src, size_t bytes)
 int32_t dbx_device_synchronize(int32_t device);
 
 /* Operator lifecycle.  `params` is the struct matching `kind`
- * (FILTER: dbx_predicate, AGG_*: dbx_agg_params, TOPK: dbx_topk_params, JOIN: dbx_join_params).
+ * (FILTER: dbx_predicate, AGG_*: dbx_agg_params, TOPK: dbx_topk_params, JOIN: dbx_join_params,
+ *  WINDOW: dbx_window_params).
  * `input_types[n_input_cols]` are the dbx_dtype of the block columns that will be pushed
  * (DataSchema of the upstream pipe); nullability is taken per block from `validity`. */
 int32_t dbx_op_create(int32_t kind, const void* params, const int32_t* input_types, int32_t n_input_cols,
